@@ -384,6 +384,16 @@ class NativeBinaryTable:
                                                              bounds.ctypes.data_as(C.POINTER(C.c_uint32))))
         return bounds
 
+    def like_bitmaps(self, column: int, pattern: bytes, condition: int) -> np.ndarray:
+        """hyb_binary_table_like_bitmaps: value_id_bounds of a LIKE predicate, the per-chunk dictionary match bitmaps."""
+        count = C.c_uint32()
+        capi.check(self.lib.hyb_binary_table_like_bitmaps(self.ptr, column, pattern, len(pattern), condition, None,
+                                                          C.byref(count)))
+        words = np.zeros(max(count.value, 1), dtype=np.uint32)
+        capi.check(self.lib.hyb_binary_table_like_bitmaps(self.ptr, column, pattern, len(pattern), condition,
+                                                          words.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(count)))
+        return words[: count.value]
+
     def host_blocks(self) -> list:
         count = C.c_uint32()
         capi.check(self.lib.hyb_binary_table_blocks(self.ptr, None, C.byref(count)))

@@ -166,6 +166,7 @@ SYMBOLS = {
     "hyb_binary_table_string_dictionary": [C.c_void_p, _U32, _U32, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)),
                                            C.POINTER(_U32)],
     "hyb_binary_table_value_id_bounds": [C.c_void_p, _U32, C.c_char_p, _U64, C.c_char_p, _U64, C.POINTER(_U32)],
+    "hyb_binary_table_like_bitmaps": [C.c_void_p, _U32, C.c_char_p, _U64, _I32, C.POINTER(_U32), C.POINTER(_U32)],
     "hyb_binary_table_blocks": [C.c_void_p, C.POINTER(HostBlock), C.POINTER(_U32)],
     "hyb_table_upload_binary": [_CTX, C.c_void_p, C.POINTER(_U64)],
     "hyb_table_info": [_CTX, _U64, C.POINTER(_U32), C.POINTER(_U32), C.POINTER(_U64), C.POINTER(_U64)],
@@ -174,6 +175,8 @@ SYMBOLS = {
     "hyb_lossless_predicate_cast": [_I32, C.POINTER(Literal), _I32, _I32, C.POINTER(_I32), C.POINTER(Value)],
     "hyb_lossless_between_cast": [_I32, C.POINTER(Literal), C.POINTER(Literal), _I32, C.POINTER(_I32), C.POINTER(Value),
                                   C.POINTER(Value)],
+    "hyb_like_dictionary_matches": [C.c_char_p, _U64, _I32, C.c_void_p, C.POINTER(_U64), _U32, C.POINTER(_U32),
+                                    C.POINTER(_U32)],
     "hyb_table_scan": [_CTX, _U64, C.POINTER(ScanPredicate), _U64, C.POINTER(_U64)],
     "hyb_pos_list_info": [_CTX, _U64, C.POINTER(_U64), C.POINTER(_U32)],
     "hyb_pos_list_chunk_offsets": [_CTX, _U64, _P],
@@ -211,6 +214,26 @@ SYMBOLS = {
     "hyb_join_result_device_ptrs": [_CTX, _U64, C.POINTER(_P), C.POINTER(_P)],
     "hyb_context_stream": [_CTX, C.POINTER(_P)],
 }
+
+
+LIKE_CONDITIONS = (PRED_LIKE, PRED_NOT_LIKE, PRED_LIKE_INSENSITIVE, PRED_NOT_LIKE_INSENSITIVE)
+
+
+def like_dictionary_matches(pattern: bytes, condition: int, entries) -> "np.ndarray":
+    """hyb_like_dictionary_matches: the LikeMatcher result of every entry of one string dictionary (a sequence of bytes)
+    as ceil(len / 32) uint32 words, entry i = bit i & 31 of word i >> 5; NOT variants are already inverted. Host only."""
+    import numpy as np
+
+    entries = [bytes(entry) for entry in entries]
+    offsets = np.zeros(len(entries) + 1, dtype=np.uint64)
+    if entries:
+        offsets[1:] = np.cumsum([len(entry) for entry in entries])
+    chars = b"".join(entries) or None  # NULL: every entry is empty
+    words = np.zeros(max((len(entries) + 31) // 32, 1), dtype=np.uint32)
+    check(load_library().hyb_like_dictionary_matches(pattern, len(pattern), condition, chars,
+                                                     offsets.ctypes.data_as(C.POINTER(C.c_uint64)), len(entries),
+                                                     words.ctypes.data_as(C.POINTER(C.c_uint32)), None))
+    return words[: (len(entries) + 31) // 32]
 
 
 IPC_HANDLE_BYTES = 64

@@ -874,7 +874,7 @@ __global__ void __launch_bounds__(kFastThreads, kMinBlocks) aggregate_fast_kerne
         if (static_cast<uint32_t>(p) < plan.predicate_count) {
           const DevSegment& segment = plan.predicate_segments[p][chunk];
           const uint32_t mode = plan.predicate_tests[p][chunk].mode;
-          early_predicate[p] = raw_codes_loadable(segment) && (mode == kTestIdRange || mode == kTestInt);
+          early_predicate[p] = raw_codes_loadable(segment) && (mode == kTestIdRange || mode == kTestIdSet || mode == kTestInt);
           raw_predicate[p] = early_predicate[p] ? load_raw_codes8(segment, row0) : uint4{0u, 0u, 0u, 0u};
         }
       }
@@ -1556,6 +1556,11 @@ static StreamLayout stream_layout_for(const Table* table, const hyb_aggregate_qu
   if (fast.work_type == 2 || table->row_count() >= 0xFFFFFFF0ull) return layout;
   // a single int32 group-by column may take the immediate-key order, which needs the LAST row of every group
   if (query->groupby_count == 1 && table->column_types[query->groupby_column_ids[0]] == HYB_TYPE_INT32) return layout;
+  // the row loop decodes a dictionary predicate as a value-ID range (predicate_mode below); LIKE needs the id-set test of
+  // the register-tile and general kernels
+  for (uint32_t p = 0; p < query->predicate_count; ++p) {
+    if (is_like_condition(query->predicates[p].condition)) return layout;
+  }
   const uint32_t chunk_count = table->chunk_count();
   std::vector<uint32_t> staged;  // distinct referenced columns
   const auto slot_of = [&](uint32_t column) -> uint32_t {

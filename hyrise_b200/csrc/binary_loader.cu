@@ -519,6 +519,36 @@ int hyb_binary_table_value_id_bounds(const hyb_binary_table* table, uint32_t col
   return HYB_OK;
 }
 
+int hyb_binary_table_like_bitmaps(const hyb_binary_table* table, uint32_t column, const char* pattern, uint64_t pattern_length,
+                                  int32_t condition, uint32_t* out_words, uint32_t* inout_word_count) {
+  HYB_CHECK(table && inout_word_count, HYB_ERR_INVALID, "NULL argument");
+  const size_t columns = table->column_types.size();
+  HYB_CHECK(column < columns && table->column_types[column] == HYB_TYPE_STRING, HYB_ERR_INVALID, "not a string column");
+  uint64_t words = 0;
+  for (size_t chunk = 0; chunk < table->chunk_rows.size(); ++chunk) {
+    const auto& dictionary = table->string_dictionaries[chunk * columns + column];
+    const uint64_t size = dictionary.offsets.empty() ? 0 : dictionary.offsets.size() - 1;
+    words += (size + 31) / 32;
+  }
+  HYB_CHECK(words <= UINT32_MAX, HYB_ERR_INVALID, "bitmap exceeds 2^32 words");
+  if (!out_words) {
+    *inout_word_count = static_cast<uint32_t>(words);
+    return HYB_OK;
+  }
+  HYB_CHECK(*inout_word_count >= words, HYB_ERR_INVALID, "out_words holds fewer words than the bitmaps need");
+  std::vector<LikeDictionary> dictionaries(table->chunk_rows.size());
+  for (size_t chunk = 0; chunk < table->chunk_rows.size(); ++chunk) {
+    const auto& dictionary = table->string_dictionaries[chunk * columns + column];
+    const uint32_t size = dictionary.offsets.empty() ? 0 : static_cast<uint32_t>(dictionary.offsets.size() - 1);
+    // chars.data() is NULL for a dictionary that holds only the empty string
+    dictionaries[chunk] = LikeDictionary{dictionary.chars.data(), dictionary.offsets.data(), size};
+  }
+  HYB_TRY(like_match_dictionaries(pattern, pattern_length, condition, dictionaries.data(), dictionaries.size(), out_words,
+                                  nullptr));
+  *inout_word_count = static_cast<uint32_t>(words);
+  return HYB_OK;
+}
+
 int hyb_table_upload_binary(hyb_context* context, const hyb_binary_table* table, hyb_table_t* out_table) {
   HYB_CHECK(context && table && out_table, HYB_ERR_INVALID, "NULL argument");
   hyb_block_set_t block_set = 0;

@@ -266,6 +266,19 @@ int fail(int status, const std::string& message);
     if (_s != HYB_OK) return _s; \
   } while (0)
 
+// LIKE over host string dictionaries (like.cu) -------------------------------------------------------------------------
+// Entry i of a dictionary = chars[offsets[i] .. offsets[i + 1]); `chars` may be NULL when every entry is empty.
+struct LikeDictionary {
+  const char* chars;
+  const uint64_t* offsets;
+  uint32_t count;
+};
+// Compiles the pattern once and writes ceil(count / 32) match words per dictionary, the dictionaries' words one after
+// another into out_words (hyb_like_dictionary_matches is the one-dictionary case).
+int like_match_dictionaries(const char* pattern, uint64_t pattern_length, int32_t condition,
+                            const LikeDictionary* dictionaries, size_t dictionary_count, uint32_t* out_words,
+                            uint64_t* out_match_count);
+
 // Helpers implemented in context.cu ---------------------------------------------------------------------------------
 class DeviceGuard {
  public:

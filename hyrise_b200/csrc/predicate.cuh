@@ -11,7 +11,8 @@ enum ChunkTestMode : uint32_t {
   kTestIdRange = 1,     // dictionary value-ID range
   kTestInt = 2,         // typed integer range (ValueSegment<int32/int64>, FrameOfReference)
   kTestFloat = 3,       // typed floating-point range (ValueSegment<float/double>)
-  kTestNull = 4         // IS NULL / IS NOT NULL on a null vector
+  kTestNull = 4,        // IS NULL / IS NOT NULL on a null vector
+  kTestIdSet = 5        // dictionary value-ID set (LIKE): match iff value_id < dict_size and its bit in id_bits is set
 };
 
 struct ChunkTest {
@@ -19,7 +20,10 @@ struct ChunkTest {
   uint32_t negate;      // NotEquals: match iff outside the range and not NULL
   uint32_t id_lo;       // kTestIdRange: match iff (value_id - id_lo) < id_span
   uint32_t id_span;
-  long long int_lo;     // kTestInt: inclusive bounds
+  union {
+    long long int_lo;         // kTestInt: inclusive bounds
+    const uint32_t* id_bits;  // kTestIdSet: device copy of the chunk's match bitmap (bit i & 31 of word i >> 5)
+  };
   long long int_hi;
   double float_lo;      // kTestFloat
   double float_hi;
@@ -28,11 +32,24 @@ struct ChunkTest {
   uint32_t want_null;   // kTestNull: 1 = IS NULL, 0 = IS NOT NULL
   uint32_t pad;
 };
+static_assert(sizeof(ChunkTest) == 64, "scan_bulk_kernel copies a test as 4 x uint4");
+
+__host__ __device__ __forceinline__ bool is_like_condition(int32_t condition) {
+  return condition >= HYB_PRED_LIKE && condition <= HYB_PRED_NOT_LIKE_INSENSITIVE;
+}
 
 
-// Builds the per-chunk tests on the device (scan.cu). Caller frees *out_tests and *out_bounds_scratch with device_free.
+// Builds the per-chunk tests (scan.cu): on the device from value-ID bounds or literals, on the host from the dictionary
+// match bitmaps of a LIKE predicate. Caller frees *out_tests and *out_bounds_scratch with device_free.
 int prepare_chunk_tests(hyb_context* context, Table* table, const hyb_scan_predicate* predicate, ChunkTest** out_tests,
                         void** out_bounds_scratch);
+
+// LIKE on a dictionary segment: value-ID `code` matches iff it is not the NULL id and its bitmap bit is set. The bitmap
+// (<= 8 KB for 65 535-entry dictionaries) is gathered through L1; a tile never straddles chunks, so a CTA reads one
+// chunk's bitmap. DESIGN.md §3.1 gives the measured cost against a value-ID range scan of the same selectivity.
+__device__ __forceinline__ bool id_set_contains(const uint32_t* bits, uint32_t dict_size, uint32_t code) {
+  return code < dict_size && ((__ldg(bits + (code >> 5)) >> (code & 31u)) & 1u);
+}
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Predicate evaluation for 8 consecutive rows of one segment. Returns a bit mask (bit j = row0 + j matches).
@@ -58,6 +75,13 @@ __device__ __forceinline__ uint32_t evaluate8(const DevSegment& segment, const C
           mask |= (!inside && codes[j] < segment.dict_size) ? (1u << j) : 0u;
         }
       }
+      break;
+    }
+    case kTestIdSet: {
+      uint32_t codes[8];
+      codes8(segment, row0, have_raw, raw, codes);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) mask |= id_set_contains(test.id_bits, segment.dict_size, codes[j]) ? (1u << j) : 0u;
       break;
     }
     case kTestInt: {
@@ -146,6 +170,9 @@ __device__ __forceinline__ bool evaluate1(const DevSegment& segment, const Chunk
       const bool inside = (code - test.id_lo) < test.id_span;
       return test.negate ? (!inside && code < segment.dict_size) : inside;
     }
+    case kTestIdSet:
+      return id_set_contains(test.id_bits, segment.dict_size,
+                             load_code1(segment.av, segment.vector_type, segment.bit_width, row));
     case kTestInt: {
       if (segment.nulls && segment.nulls[row]) return false;
       long long value;

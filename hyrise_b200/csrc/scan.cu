@@ -653,6 +653,10 @@ __device__ __forceinline__ uint32_t evaluate8_staged(const DevSegment& segment, 
         }
       }
       break;
+    case kTestIdSet:
+#pragma unroll
+      for (int j = 0; j < 8; ++j) mask |= id_set_contains(test.id_bits, segment.dict_size, codes[j]) ? (1u << j) : 0u;
+      break;
     case kTestInt: {
       uint32_t minimum = 0;
       if (segment.encoding == HYB_ENC_FRAME_OF_REFERENCE) {
@@ -954,8 +958,66 @@ __global__ void pos_list_chunk_ends_kernel(const hyb_row_id* __restrict__ rows, 
 }
 
 static bool supported_condition(int32_t condition) {
-  return (condition >= HYB_PRED_EQUALS && condition <= HYB_PRED_BETWEEN_EXCLUSIVE) || condition == HYB_PRED_IS_NULL ||
-         condition == HYB_PRED_IS_NOT_NULL;
+  return (condition >= HYB_PRED_EQUALS && condition <= HYB_PRED_BETWEEN_EXCLUSIVE) || is_like_condition(condition) ||
+         condition == HYB_PRED_IS_NULL || condition == HYB_PRED_IS_NOT_NULL;
+}
+
+// LIKE: the caller's per-chunk dictionary match bitmaps (ColumnLikeTableScanImpl::_find_matches_in_dictionary,
+// column_like_table_scan_impl.cpp:75-140) become per-chunk tests on the host, which reads the bitmaps anyway. No bit set:
+// kTestNone (the chunk's bytes are skipped); one contiguous run of set bits (every entry, or a prefix pattern on a sorted
+// dictionary): kTestIdRange, as fast as a range scan; anything else: kTestIdSet, and only those chunks' words are uploaded.
+static int prepare_like_tests(hyb_context* context, Table* table, const hyb_scan_predicate* predicate, void* tests,
+                              void** out_bitmap_scratch) {
+  const uint32_t chunk_count = table->chunk_count();
+  std::vector<ChunkTest> host(chunk_count);
+  std::vector<uint32_t> set_words;
+  size_t word = 0;
+  for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+    const DevSegment& segment = table->segments[size_t{chunk} * table->column_count + predicate->column_id];
+    const uint32_t size = segment.dict_size;
+    const uint32_t* bits = predicate->value_id_bounds + word;
+    word += (size_t{size} + 31) / 32;
+    ChunkTest& test = host[chunk];
+    test = ChunkTest{};
+    test.mode = kTestNone;
+    if (segment.row_count == 0) continue;
+    HYB_CHECK(segment.encoding == HYB_ENC_DICTIONARY, HYB_ERR_INVALID, "LIKE needs dictionary-encoded string segments");
+    uint32_t count = 0, first = 0, last = 0;
+    for (uint32_t w = 0; w < (size + 31) / 32; ++w) {
+      uint32_t bits_w = bits[w];
+      if (w == size / 32) bits_w &= (1u << (size & 31)) - 1u;  // padding bits of the last word are ignored
+      if (!bits_w) continue;
+      if (count == 0) first = 32 * w + static_cast<uint32_t>(__builtin_ctz(bits_w));
+      last = 32 * w + 31 - static_cast<uint32_t>(__builtin_clz(bits_w));
+      count += static_cast<uint32_t>(__builtin_popcount(bits_w));
+    }
+    if (count == 0) continue;
+    if (last - first + 1 == count) {
+      test.mode = kTestIdRange;
+      test.id_lo = first;
+      test.id_span = count;
+    } else {
+      test.mode = kTestIdSet;
+      test.int_hi = static_cast<long long>(set_words.size());  // word offset until the scratch address is known
+      set_words.insert(set_words.end(), bits, bits + (size + 31) / 32);
+    }
+  }
+  if (!set_words.empty()) {
+    HYB_TRY(device_alloc(context, sizeof(uint32_t) * set_words.size(), out_bitmap_scratch));
+    const auto* base = static_cast<const uint32_t*>(*out_bitmap_scratch);
+    for (auto& test : host) {
+      if (test.mode != kTestIdSet) continue;
+      test.id_bits = base + test.int_hi;
+      test.int_hi = 0;
+    }
+    // pageable sources: both copies are staged before cudaMemcpyAsync returns
+    HYB_CUDA(cudaMemcpyAsync(*out_bitmap_scratch, set_words.data(), sizeof(uint32_t) * set_words.size(),
+                             cudaMemcpyHostToDevice, context->stream));
+  }
+  if (chunk_count) {
+    HYB_CUDA(cudaMemcpyAsync(tests, host.data(), sizeof(ChunkTest) * chunk_count, cudaMemcpyHostToDevice, context->stream));
+  }
+  return HYB_OK;
 }
 
 // Shared by hyb_table_scan and the fused predicates of hyb_aggregate_hash: builds the per-chunk tests on the device.
@@ -970,6 +1032,23 @@ int prepare_chunk_tests(hyb_context* context, Table* table, const hyb_scan_predi
   const int32_t data_type = table->column_types[predicate->column_id];
   const bool needs_value =
       predicate->condition != HYB_PRED_IS_NULL && predicate->condition != HYB_PRED_IS_NOT_NULL;
+  if (is_like_condition(predicate->condition)) {
+    // table_scan.cpp creates a ColumnLikeTableScanImpl only for string columns (ScanLikeNonStringColumn)
+    HYB_CHECK(data_type == HYB_TYPE_STRING, HYB_ERR_INVALID, "LIKE needs a string column");
+    HYB_CHECK(predicate->value_id_bounds, HYB_ERR_INVALID,
+              "LIKE scans need host-computed dictionary match bitmaps in value_id_bounds (hyb_like_dictionary_matches)");
+    void* tests = nullptr;
+    HYB_TRY(device_alloc(context, sizeof(ChunkTest) * std::max<uint32_t>(chunk_count, 1), &tests));
+    const int status = prepare_like_tests(context, table, predicate, tests, out_bounds_scratch);
+    if (status != HYB_OK) {
+      device_free(context, tests);
+      device_free(context, *out_bounds_scratch);
+      *out_bounds_scratch = nullptr;
+      return status;
+    }
+    *out_tests = static_cast<ChunkTest*>(tests);
+    return HYB_OK;
+  }
   if (data_type == HYB_TYPE_STRING && needs_value) {
     HYB_CHECK(predicate->value_id_bounds, HYB_ERR_INVALID,
               "string dictionary scans need host-computed value_id_bounds (dictionary_segment.cpp:94-119)");

@@ -20,9 +20,10 @@ ROW_ID_DTYPE = np.dtype([("chunk_id", np.uint32), ("chunk_offset", np.uint32)])
 
 @dataclass
 class Predicate:
-    """column <condition> value | column BETWEEN lower AND upper | column IS [NOT] NULL — the arguments of
-    ColumnVsValueTableScanImpl / ColumnBetweenTableScanImpl / ColumnIsNullTableScanImpl after
-    lossless_predicate_variant_cast (table_scan.cpp:340-366)."""
+    """column <condition> value | column BETWEEN lower AND upper | column IS [NOT] NULL | column [NOT] LIKE pattern — the
+    arguments of ColumnVsValueTableScanImpl / ColumnBetweenTableScanImpl / ColumnIsNullTableScanImpl after
+    lossless_predicate_variant_cast (table_scan.cpp:340-366), or of ColumnLikeTableScanImpl with the pattern (bytes or
+    str) in `lower`."""
 
     column_id: int
     condition: int
@@ -51,8 +52,16 @@ def build_scan_predicate(table: Table, predicate: Predicate) -> tuple[capi.ScanP
     struct.condition = predicate.condition
     keepalive = None
     needs_value = predicate.condition not in (capi.PRED_IS_NULL, capi.PRED_IS_NOT_NULL)
+    if predicate.condition in capi.LIKE_CONDITIONS and data_type != capi.TYPE_STRING:
+        # ScanLikeNonStringColumn (table_scan_string_test.cpp): LIKE on a non-string column is an error, not a CPU job
+        raise capi.HyriseB200Error(capi.HYB_ERR_INVALID, "LIKE needs a string column")
     if data_type == capi.TYPE_STRING:
-        if needs_value:
+        if predicate.condition in capi.LIKE_CONDITIONS:
+            bitmaps = table.string_like_bitmaps(predicate)
+            keepalive = np.zeros(max(bitmaps.size, 1), dtype=np.uint32)  # never NULL, even without dictionary entries
+            keepalive[: bitmaps.size] = bitmaps
+            struct.value_id_bounds = keepalive.ctypes.data
+        elif needs_value:
             keepalive = np.ascontiguousarray(table.string_value_id_bounds(predicate), dtype=np.uint32)
             struct.value_id_bounds = keepalive.ctypes.data
     else:

@@ -362,6 +362,16 @@ class Table:
                         else position
         return bounds
 
+    def string_like_bitmaps(self, predicate) -> np.ndarray:
+        """value_id_bounds of a LIKE predicate: per chunk, the dictionary match bitmap of ColumnLikeTableScanImpl
+        (column_like_table_scan_impl.cpp:75-140) from hyb_like_dictionary_matches, ceil(dictionary size / 32) uint32 words
+        per chunk in chunk order. The pattern is `predicate.lower` (bytes, or str encoded as UTF-8)."""
+        pattern = predicate.lower if isinstance(predicate.lower, bytes) else str(predicate.lower).encode()
+        words = [capi.like_dictionary_matches(pattern, predicate.condition,
+                                              chunk.segments[predicate.column_id].string_dictionary)
+                 for chunk in self.chunks]
+        return np.concatenate(words) if words else np.zeros(0, dtype=np.uint32)
+
     def column_values(self, column_id: int) -> tuple[np.ndarray, np.ndarray]:
         """Decoded values and null mask of a whole column (host side)."""
         if not self.chunks:

@@ -23,7 +23,7 @@
  *   - plain C: pointers + sizes, no C++/torch types; every function returns hyb_status (0 = OK);
  *     hyb_last_error() returns a thread-local message. No exception crosses this boundary.
  *   - every entry point is thread-safe and re-entrant; inputs are borrowed and immutable for the duration of the call.
- *   - HYB_ERR_UNSUPPORTED means "run the CPU operator" (e.g. LIKE scans, string join keys); anything else is a
+ *   - HYB_ERR_UNSUPPORTED means "run the CPU operator" (e.g. IN scans, string join keys); anything else is a
  *     hard failure the shim turns into Fail(hyb_last_error()).
  *   - results stay device-resident behind handles (so the next operator can consume them without a PCIe round trip)
  *     and are copied out on request into caller-owned host memory (pinned via hyb_host_alloc for full PCIe speed).
@@ -104,10 +104,10 @@ typedef enum hyb_predicate_condition {
   HYB_PRED_BETWEEN_EXCLUSIVE = 9,
   HYB_PRED_IN = 10,                   /* unsupported */
   HYB_PRED_NOT_IN = 11,               /* unsupported */
-  HYB_PRED_LIKE = 12,                 /* unsupported */
-  HYB_PRED_NOT_LIKE = 13,             /* unsupported */
-  HYB_PRED_LIKE_INSENSITIVE = 14,     /* unsupported */
-  HYB_PRED_NOT_LIKE_INSENSITIVE = 15, /* unsupported */
+  HYB_PRED_LIKE = 12,                 /* STRING dictionary columns: value_id_bounds = match bitmaps */
+  HYB_PRED_NOT_LIKE = 13,             /* STRING dictionary columns: value_id_bounds = match bitmaps */
+  HYB_PRED_LIKE_INSENSITIVE = 14,     /* STRING dictionary columns: value_id_bounds = match bitmaps */
+  HYB_PRED_NOT_LIKE_INSENSITIVE = 15, /* STRING dictionary columns: value_id_bounds = match bitmaps */
   HYB_PRED_IS_NULL = 16,
   HYB_PRED_IS_NOT_NULL = 17
 } hyb_predicate_condition;
@@ -257,6 +257,12 @@ int hyb_binary_table_string_dictionary(const hyb_binary_table* table, uint32_t c
 int hyb_binary_table_value_id_bounds(const hyb_binary_table* table, uint32_t column, const char* value, uint64_t value_length,
                                      const char* value2, uint64_t value2_length, uint32_t* out_bounds);
 
+/* value_id_bounds of a LIKE predicate on a string column of this table: the per-chunk dictionary match bitmaps
+ * (hyb_like_dictionary_matches over every chunk's dictionary, concatenated in chunk order). out_words == NULL: only
+ * *inout_word_count is set, to the number of words needed; otherwise *inout_word_count must be at least that. */
+int hyb_binary_table_like_bitmaps(const hyb_binary_table* table, uint32_t column, const char* pattern, uint64_t pattern_length,
+                                  int32_t condition, uint32_t* out_words, uint32_t* inout_word_count);
+
 /*
  * Arena upload: when the segment buffers of one or more tables live inside a few large host blocks (a pinned
  * MemoryResource arena, cf. src/lib/memory/default_memory_resource.cpp:29-35 and Chunk::migrate, storage/chunk.hpp:119),
@@ -294,6 +300,13 @@ int hyb_table_info(hyb_context* context, hyb_table_t table, uint32_t* out_chunk_
  *                                                                                                           (between)
  * with HYB_INVALID_VALUE_ID for "past the end". For numeric dictionaries leave it NULL: bounds are computed on the
  * device from `lower`/`upper`.
+ * LIKE / NOT LIKE / LIKE INSENSITIVE / NOT LIKE INSENSITIVE (STRING columns only, HYB_ERR_INVALID otherwise):
+ * value_id_bounds points to the per-chunk dictionary match bitmaps, the ColumnLikeTableScanImpl's dictionary path
+ * (column_like_table_scan_impl.cpp:75-140). Chunk c contributes ceil(dictionary_size_c / 32) words, chunks follow one
+ * another in chunk order, and entry i of a chunk's dictionary is bit (i & 31) of its word (i >> 5). A bit is the
+ * matcher's result, so NOT variants pass the inverted matches (hyb_like_dictionary_matches computes them). Padding bits
+ * are ignored, and the NULL value-ID (== dictionary_size) never matches. Chunks whose bitmap has no bit set are skipped,
+ * one contiguous run of set bits scans like a value-ID range, any other set is looked up per row.
  */
 typedef struct hyb_scan_predicate {
   uint32_t column_id;
@@ -323,6 +336,19 @@ int hyb_lossless_predicate_cast(int32_t condition, const hyb_literal* literal, i
                                 int32_t* out_condition, hyb_value* out_value);
 int hyb_lossless_between_cast(int32_t condition, const hyb_literal* lower, const hyb_literal* upper, int32_t column_type,
                               int32_t* out_condition, hyb_value* out_lower, hyb_value* out_upper);
+
+/*
+ * LikeMatcher (expression/evaluation/like_matcher.{hpp,cpp}) over one string dictionary (host only, no GPU): entry i =
+ * chars[offsets[i] .. offsets[i + 1]); chars may be NULL when every entry is the empty string. out_words receives ceil(count / 32) words, bit (i & 31) of word (i >> 5) set iff
+ * entry i satisfies `pattern` under `condition` (one of the four LIKE conditions; NOT variants invert), padding bits
+ * cleared; out_match_count (optional) the number of set bits. `_` is one character and `%` any run; there is no escape
+ * character. Patterns of the forms abc%, %abc, %abc% and %a%b%... are matched directly; any other becomes the
+ * reference's anchored ECMAScript regular expression, whose `_` and `%` do not match '\n' or '\r'. INSENSITIVE lowers
+ * A-Z of pattern and entries (std::tolower in the C locale). HYB_ERR_INVALID: not a LIKE condition, or a pattern that
+ * is no valid regular expression (an unbalanced `[`), which the reference rejects as well.
+ */
+int hyb_like_dictionary_matches(const char* pattern, uint64_t pattern_length, int32_t condition, const char* chars,
+                                const uint64_t* offsets, uint32_t count, uint32_t* out_words, uint32_t* out_match_count);
 
 /*
  * Scan `table` and produce, per input chunk, the ascending list of matching RowIDs — what

@@ -18,6 +18,7 @@
 // can feed the next operator (a TableScan's PosList as the filter of a JoinHash / AggregateHash / second TableScan).
 #pragma once
 
+#include <algorithm>
 #include <cstdint>
 #include <memory>
 #include <optional>
@@ -71,7 +72,7 @@ enum class WindowFunction : int32_t {  // expression/window_function_expression.
   CountStar = HYB_AGG_COUNT_STAR
 };
 
-// HYB_ERR_UNSUPPORTED: the caller runs the reference's CPU operator instead (LIKE scans, string join keys, ...).
+// HYB_ERR_UNSUPPORTED: the caller runs the reference's CPU operator instead (IN scans, string join keys, ...).
 class UnsupportedOnDevice : public std::logic_error {
  public:
   using std::logic_error::logic_error;
@@ -134,6 +135,15 @@ class BinaryTable {
     check(hyb_binary_table_value_id_bounds(_table, column, value.data(), value.size(), value2 ? value2->data() : nullptr,
                                            value2 ? value2->size() : 0, bounds.data()));
     return bounds;
+  }
+  // hyb_scan_predicate.value_id_bounds of a LIKE predicate: the per-chunk dictionary match bitmaps (LikeMatcher over every
+  // chunk's dictionary, column_like_table_scan_impl.cpp:75-140)
+  std::vector<uint32_t> like_value_id_bitmaps(uint32_t column, const std::string& pattern, int32_t condition) const {
+    uint32_t words = 0;
+    check(hyb_binary_table_like_bitmaps(_table, column, pattern.data(), pattern.size(), condition, nullptr, &words));
+    std::vector<uint32_t> bitmaps(std::max<uint32_t>(words, 1));
+    check(hyb_binary_table_like_bitmaps(_table, column, pattern.data(), pattern.size(), condition, bitmaps.data(), &words));
+    return bitmaps;
   }
 
  private:
@@ -313,7 +323,9 @@ struct ScanPredicate {
   PredicateCondition condition;
   std::optional<AllTypeVariant> value;   // binary conditions and the lower bound of BETWEEN
   std::optional<AllTypeVariant> value2;  // upper bound of BETWEEN
-  std::vector<uint32_t> string_value_id_bounds;  // string dictionaries: per-chunk bounds, see hyb_scan_predicate
+  // string dictionaries: per-chunk bounds; for the LIKE conditions the per-chunk dictionary match bitmaps
+  // (BinaryTable::like_value_id_bitmaps, hyb_like_dictionary_matches); see hyb_scan_predicate
+  std::vector<uint32_t> string_value_id_bounds;
 
   // The predicate with its literal(s) cast to `column_type`; nullopt: no lossless form (run the CPU operator).
   std::optional<ScanPredicate> normalized(DataType column_type) const {

@@ -3,6 +3,7 @@
 #include <atomic>
 
 #include "device_column_pool.hpp"
+#include "expression/evaluation/like_matcher.hpp"
 #include "expression/expression_utils.hpp"
 #include "expression/pqp_column_expression.hpp"
 #include "expression/window_function_expression.hpp"
@@ -10,6 +11,7 @@
 #include "operators/join_helper/join_output_writing.hpp"
 #include "resolve_type.hpp"
 #include "storage/dictionary_segment.hpp"
+#include "storage/fixed_string_dictionary_segment.hpp"
 #include "storage/pos_lists/row_id_pos_list.hpp"
 #include "storage/reference_segment.hpp"
 #include "storage/value_segment.hpp"
@@ -73,6 +75,35 @@ bool string_value_id_bounds(const Table& stored, ColumnID column_id, const AllTy
   return true;
 }
 
+// ColumnLikeTableScanImpl's dictionary path (column_like_table_scan_impl.cpp:75-140) for every chunk at once: the
+// reference's own LikeMatcher over each dictionary, one bit per entry, ceil(size / 32) words per chunk in chunk order.
+bool like_dictionary_bitmaps(const Table& stored, ColumnID column_id, PredicateCondition condition, const pmr_string& pattern,
+                             std::vector<uint32_t>& words) {
+  const auto matcher = LikeMatcher{pattern, condition};
+  for (auto chunk_id = ChunkID{0}; chunk_id < stored.chunk_count(); ++chunk_id) {
+    const auto segment = stored.get_chunk(chunk_id)->get_segment(column_id);
+    const auto append = [&](const size_t size, const auto& entry_at) {
+      const auto first = words.size();
+      words.resize(first + (size + 31) / 32, 0);
+      matcher.resolve([&](const auto& predicate) {
+        for (auto entry = size_t{0}; entry < size; ++entry) {
+          words[first + entry / 32] |= predicate(entry_at(entry)) ? (1u << (entry % 32)) : 0u;
+        }
+      });
+    };
+    if (const auto dictionary_segment = std::dynamic_pointer_cast<const DictionarySegment<pmr_string>>(segment)) {
+      const auto& dictionary = *dictionary_segment->dictionary();
+      append(dictionary.size(), [&](const size_t entry) -> const pmr_string& { return dictionary[entry]; });
+    } else if (const auto fixed_segment = std::dynamic_pointer_cast<const FixedStringDictionarySegment<pmr_string>>(segment)) {
+      const auto& dictionary = *fixed_segment->fixed_string_dictionary();
+      append(dictionary.size(), [&](const size_t entry) { return dictionary.get_string_at(entry); });
+    } else {
+      return false;
+    }
+  }
+  return true;
+}
+
 // PosLists of a device result -> one output chunk of ReferenceSegments per input chunk with matches (table_scan.cpp:199-217).
 std::shared_ptr<const Table> wrap_pos_lists(hyb_context* context, const std::shared_ptr<const Table>& stored, hyb_pos_list_t result) {
   auto chunk_count = uint32_t{0};
@@ -128,7 +159,16 @@ std::shared_ptr<const Table> try_gpu_table_scan(const std::shared_ptr<const Tabl
   predicate.condition = static_cast<int32_t>(condition);  // PredicateCondition and hyb_predicate_condition share values
   auto bounds = std::vector<uint32_t>{};
   const auto needs_value = condition != PredicateCondition::IsNull && condition != PredicateCondition::IsNotNull;
-  if (needs_value && column_type == DataType::String) {
+  const auto is_like = condition == PredicateCondition::Like || condition == PredicateCondition::NotLike ||
+                       condition == PredicateCondition::LikeInsensitive || condition == PredicateCondition::NotLikeInsensitive;
+  if (is_like) {
+    if (column_type != DataType::String ||
+        !like_dictionary_bitmaps(*in_table, column_id, condition, boost::get<pmr_string>(value), bounds)) {
+      return nullptr;  // the reference operator reports LIKE on a non-string column itself
+    }
+    bounds.push_back(0);  // never a NULL pointer, even when no chunk has a dictionary entry
+    predicate.value_id_bounds = bounds.data();
+  } else if (needs_value && column_type == DataType::String) {
     if (!string_value_id_bounds(*in_table, column_id, value, value2, bounds)) {
       return nullptr;
     }
