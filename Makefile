@@ -12,7 +12,9 @@ HDRS      := $(wildcard $(CSRC)/*.hpp) $(wildcard $(CSRC)/*.cuh) include/hyrise_
 
 TPCH_LIB  := hyrise_b200/lib/libhyb_tpch.so
 
-all: $(LIB) $(TPCH_LIB) oracle
+COLUMN_SCAN_ORACLE := build/libcolumn_scan_oracle.so
+
+all: $(LIB) $(TPCH_LIB) oracle $(COLUMN_SCAN_ORACLE)
 
 build/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p build
@@ -41,6 +43,18 @@ build/predicate_cast_check: tests/cpp/predicate_cast_check.cpp include/hyrise_b2
 	@mkdir -p build
 	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/predicate_cast_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
 		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
+
+# Column-vs-column TableScan through the mirror on the GPU (one string and one numeric comparison).
+build/column_scan_check: tests/cpp/column_scan_check.cpp include/hyrise_b200.hpp include/hyrise_b200.h $(LIB)
+	@mkdir -p build
+	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/column_scan_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
+		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
+
+# CPU restatement of ColumnVsColumnTableScanImpl on decoded numeric values (test infrastructure, tests/column_scan_oracle.py).
+# No -ffast-math: the comparisons must follow IEEE and C++'s arithmetic conversions exactly.
+$(COLUMN_SCAN_ORACLE): tests/cpp/column_scan_oracle.cpp include/hyrise_b200.h
+	@mkdir -p build
+	$(CXX) -O2 -std=c++17 -fPIC -Wall -Wextra -shared -o $@ tests/cpp/column_scan_oracle.cpp
 
 clean:
 	rm -rf build $(LIB) $(TPCH_LIB)

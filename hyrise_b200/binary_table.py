@@ -394,6 +394,16 @@ class NativeBinaryTable:
                                                           words.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(count)))
         return words[: count.value]
 
+    def column_translation(self, left_column: int, right_column: int) -> np.ndarray:
+        """hyb_binary_table_column_translation: right_in_left of a column-vs-column scan on two string columns."""
+        count = C.c_uint32()
+        capi.check(self.lib.hyb_binary_table_column_translation(self.ptr, left_column, right_column, None, C.byref(count)))
+        words = np.zeros(max(count.value, 1), dtype=np.uint32)
+        capi.check(self.lib.hyb_binary_table_column_translation(self.ptr, left_column, right_column,
+                                                                words.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                                                C.byref(count)))
+        return words[: count.value]
+
     def host_blocks(self) -> list:
         count = C.c_uint32()
         capi.check(self.lib.hyb_binary_table_blocks(self.ptr, None, C.byref(count)))

@@ -85,6 +85,16 @@ class ScanPredicate(C.Structure):
     ]
 
 
+class ColumnScanPredicate(C.Structure):
+    _fields_ = [
+        ("left_column_id", C.c_uint32),
+        ("condition", C.c_int32),
+        ("right_column_id", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("right_in_left", C.c_void_p),
+    ]
+
+
 class Literal(C.Structure):
     _fields_ = [("data_type", C.c_int32), ("value", Value)]
 
@@ -167,6 +177,7 @@ SYMBOLS = {
                                            C.POINTER(_U32)],
     "hyb_binary_table_value_id_bounds": [C.c_void_p, _U32, C.c_char_p, _U64, C.c_char_p, _U64, C.POINTER(_U32)],
     "hyb_binary_table_like_bitmaps": [C.c_void_p, _U32, C.c_char_p, _U64, _I32, C.POINTER(_U32), C.POINTER(_U32)],
+    "hyb_binary_table_column_translation": [C.c_void_p, _U32, _U32, C.POINTER(_U32), C.POINTER(_U32)],
     "hyb_binary_table_blocks": [C.c_void_p, C.POINTER(HostBlock), C.POINTER(_U32)],
     "hyb_table_upload_binary": [_CTX, C.c_void_p, C.POINTER(_U64)],
     "hyb_table_info": [_CTX, _U64, C.POINTER(_U32), C.POINTER(_U32), C.POINTER(_U64), C.POINTER(_U64)],
@@ -177,7 +188,9 @@ SYMBOLS = {
                                   C.POINTER(Value)],
     "hyb_like_dictionary_matches": [C.c_char_p, _U64, _I32, C.c_void_p, C.POINTER(_U64), _U32, C.POINTER(_U32),
                                     C.POINTER(_U32)],
+    "hyb_dictionary_translate": [C.c_void_p, C.POINTER(_U64), _U32, C.c_void_p, C.POINTER(_U64), _U32, C.POINTER(_U32)],
     "hyb_table_scan": [_CTX, _U64, C.POINTER(ScanPredicate), _U64, C.POINTER(_U64)],
+    "hyb_table_scan_columns": [_CTX, _U64, C.POINTER(ColumnScanPredicate), _U64, C.POINTER(_U64)],
     "hyb_pos_list_info": [_CTX, _U64, C.POINTER(_U64), C.POINTER(_U32)],
     "hyb_pos_list_chunk_offsets": [_CTX, _U64, _P],
     "hyb_pos_list_copy": [_CTX, _U64, _U64, _U64, _P],
@@ -234,6 +247,33 @@ def like_dictionary_matches(pattern: bytes, condition: int, entries) -> "np.ndar
                                                      offsets.ctypes.data_as(C.POINTER(C.c_uint64)), len(entries),
                                                      words.ctypes.data_as(C.POINTER(C.c_uint32)), None))
     return words[: (len(entries) + 31) // 32]
+
+
+def _string_dictionary_arguments(entries) -> tuple:
+    """(chars or None, uint64 offsets) of a sequence of bytes in the layout of the dictionary entry points."""
+    import numpy as np
+
+    entries = [bytes(entry) for entry in entries]
+    offsets = np.zeros(len(entries) + 1, dtype=np.uint64)
+    if entries:
+        offsets[1:] = np.cumsum([len(entry) for entry in entries])
+    return b"".join(entries) or None, offsets  # NULL characters: every entry is empty
+
+
+def dictionary_translate(left_entries, right_entries) -> "np.ndarray":
+    """hyb_dictionary_translate: right_in_left of one chunk, for two sorted unique string dictionaries (sequences of
+    bytes): word j = 2 * lower_bound(left, right[j]) + (right[j] in left). Host only."""
+    import numpy as np
+
+    left_chars, left_offsets = _string_dictionary_arguments(left_entries)
+    right_chars, right_offsets = _string_dictionary_arguments(right_entries)
+    count = len(right_offsets) - 1
+    words = np.zeros(max(count, 1), dtype=np.uint32)
+    check(load_library().hyb_dictionary_translate(left_chars, left_offsets.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                  len(left_offsets) - 1, right_chars,
+                                                  right_offsets.ctypes.data_as(C.POINTER(C.c_uint64)), count,
+                                                  words.ctypes.data_as(C.POINTER(C.c_uint32))))
+    return words[:count]
 
 
 IPC_HANDLE_BYTES = 64

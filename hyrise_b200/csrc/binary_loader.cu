@@ -549,6 +549,37 @@ int hyb_binary_table_like_bitmaps(const hyb_binary_table* table, uint32_t column
   return HYB_OK;
 }
 
+int hyb_binary_table_column_translation(const hyb_binary_table* table, uint32_t left_column, uint32_t right_column,
+                                        uint32_t* out_words, uint32_t* inout_count) {
+  HYB_CHECK(table && inout_count, HYB_ERR_INVALID, "NULL argument");
+  const size_t columns = table->column_types.size();
+  HYB_CHECK(left_column < columns && table->column_types[left_column] == HYB_TYPE_STRING && right_column < columns &&
+                table->column_types[right_column] == HYB_TYPE_STRING,
+            HYB_ERR_INVALID, "not two string columns");
+  const auto view = [&](size_t chunk, uint32_t column) {
+    const auto& dictionary = table->string_dictionaries[chunk * columns + column];
+    const uint32_t size = dictionary.offsets.empty() ? 0 : static_cast<uint32_t>(dictionary.offsets.size() - 1);
+    // chars.data() is NULL for a dictionary that holds only the empty string
+    return LikeDictionary{dictionary.chars.data(), dictionary.offsets.data(), size};
+  };
+  uint64_t words = 0;
+  for (size_t chunk = 0; chunk < table->chunk_rows.size(); ++chunk) words += view(chunk, right_column).count;
+  HYB_CHECK(words <= UINT32_MAX, HYB_ERR_INVALID, "translation exceeds 2^32 words");
+  if (!out_words) {
+    *inout_count = static_cast<uint32_t>(words);
+    return HYB_OK;
+  }
+  HYB_CHECK(*inout_count >= words, HYB_ERR_INVALID, "out_words holds fewer words than the translation needs");
+  uint32_t* at = out_words;
+  for (size_t chunk = 0; chunk < table->chunk_rows.size(); ++chunk) {
+    const LikeDictionary right = view(chunk, right_column);
+    HYB_TRY(translate_dictionary(view(chunk, left_column), right, at));
+    at += right.count;
+  }
+  *inout_count = static_cast<uint32_t>(words);
+  return HYB_OK;
+}
+
 int hyb_table_upload_binary(hyb_context* context, const hyb_binary_table* table, hyb_table_t* out_table) {
   HYB_CHECK(context && table && out_table, HYB_ERR_INVALID, "NULL argument");
   hyb_block_set_t block_set = 0;

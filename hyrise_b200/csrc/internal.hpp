@@ -278,6 +278,9 @@ struct LikeDictionary {
 int like_match_dictionaries(const char* pattern, uint64_t pattern_length, int32_t condition,
                             const LikeDictionary* dictionaries, size_t dictionary_count, uint32_t* out_words,
                             uint64_t* out_match_count);
+// hyb_dictionary_translate (translate.cu): right_in_left of one chunk, right.count words, for two sorted unique
+// dictionaries in the layout above.
+int translate_dictionary(const LikeDictionary& left, const LikeDictionary& right, uint32_t* out_words);
 
 // Helpers implemented in context.cu ---------------------------------------------------------------------------------
 class DeviceGuard {

@@ -17,12 +17,18 @@
 //                         (chunk by chunk, ascending ChunkOffset), in a single pass over the input.
 //
 // HBM traffic per launch = N * (bytes per row of the scanned column) + M * 8 (RowIDs) — the compulsory bytes.
+//
+// Column-vs-column predicates (hyb_table_scan_columns, ColumnVsColumnTableScanImpl) run through the same two-pass and
+// position-filtered kernels: scan_mask_kernel and filtered_scan_kernel are templates on the row evaluator (ColumnRows:
+// one column against its ChunkTest; PairRows: two columns against a PairTest, column_pair.cuh).
 #include <algorithm>
+#include <cstdio>
 #include <cstdlib>
 #include <cmath>
 #include <limits>
 
 #include "bulk_copy.cuh"
+#include "column_pair.cuh"
 #include "device_utils.cuh"
 #include "internal.hpp"
 #include "predicate.cuh"
@@ -458,9 +464,61 @@ __global__ void __launch_bounds__(kScanThreads) scan_kernel(const ScanParams par
 //   scan_expand_kernel  turns the bits into RowIDs at the tile's known output offset: warp scan, staging in shared memory,
 //                       coalesced stores — scan_kernel without its loads, its predicate and its look-back chain.
 // Traffic: column + 2 x rows / 8 + RowIDs, i.e. ~5 % more than the single pass; the kernels are plain streaming kernels.
+//
+// Row evaluators: scan_mask_kernel and filtered_scan_kernel take the chunk's test through `Rows`. `Extra` is what the
+// evaluator needs beyond ScanParams / FilteredScanParams; it is the kernels' LAST parameter, so the one-column kernels
+// (empty Extra) keep their parameter layout and code.
 // ---------------------------------------------------------------------------------------------------------------------
+struct ColumnRows {  // <column> <predicate>: the chunk's ChunkTest
+  struct Extra {};
+  struct Chunk {
+    DevSegment segment;
+    ChunkTest test;
+  };
+  static __device__ __forceinline__ Chunk chunk(const ScanParams& params, const Extra&, uint32_t chunk) {
+    return Chunk{params.segments[chunk], params.tests[chunk]};
+  }
+  static __device__ __forceinline__ uint32_t mask8(const Chunk& state, uint32_t row0) {
+    return (state.test.mode != kTestNone && row0 < state.segment.row_count) ? evaluate8(state.segment, state.test, row0)
+                                                                            : 0u;
+  }
+  static __device__ __forceinline__ bool test1(const DevSegment* segments, const ChunkTest* tests, const Extra&,
+                                               uint32_t chunk, uint32_t row) {
+    const DevSegment& segment = segments[chunk];
+    const ChunkTest& test = tests[chunk];
+    return evaluate1(segment, test, row);
+  }
+};
+
+struct PairRows {  // <left column> <condition> <right column>: the params' segments are the left column's
+  struct Extra {
+    const DevSegment* right_segments;  // descriptors of the right column, one per chunk
+    const PairTest* tests;             // per chunk
+  };
+  struct Chunk {
+    DevSegment left, right;
+    PairTest test;
+  };
+  static __device__ __forceinline__ Chunk chunk(const ScanParams& params, const Extra& extra, uint32_t chunk) {
+    return Chunk{params.segments[chunk], extra.right_segments[chunk], extra.tests[chunk]};
+  }
+  static __device__ __forceinline__ uint32_t mask8(const Chunk& state, uint32_t row0) {
+    return (state.test.mode != kPairNone && row0 < state.left.row_count)
+               ? evaluate8_pair(state.left, state.right, state.test, row0)
+               : 0u;
+  }
+  static __device__ __forceinline__ bool test1(const DevSegment* segments, const ChunkTest*, const Extra& extra,
+                                               uint32_t chunk, uint32_t row) {
+    const PairTest& test = extra.tests[chunk];
+    if (test.mode == kPairNone) return false;
+    return evaluate1_pair(segments[chunk], extra.right_segments[chunk], test, row);
+  }
+};
+
+template <typename Rows>
 __global__ void __launch_bounds__(kScanThreads) scan_mask_kernel(const ScanParams params, uint32_t* __restrict__ masks_out,
-                                                                 uint32_t* __restrict__ tile_counts) {
+                                                                 uint32_t* __restrict__ tile_counts,
+                                                                 const typename Rows::Extra extra) {
   __shared__ uint32_t s_warp_totals[kScanWarps];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // Two tiles per iteration: their 2 x 4 vector loads per thread are independent and all in flight before the first
@@ -473,12 +531,11 @@ __global__ void __launch_bounds__(kScanThreads) scan_mask_kernel(const ScanParam
       if (tiles[t] >= params.tile_count) continue;  // uniform
       const uint2 info = __ldg(params.tile_map + tiles[t]);
       const uint32_t chunk = info.x, tile_row0 = info.y & 0x7FFFFFFFu;
-      const DevSegment segment = params.segments[chunk];
-      const ChunkTest test = params.tests[chunk];
+      const typename Rows::Chunk state = Rows::chunk(params, extra, chunk);
 #pragma unroll
       for (int it = 0; it < kScanIterations; ++it) {
         const uint32_t row0 = tile_row0 + warp * kScanWarpRows + it * 256 + lane * 8;
-        const uint32_t mask = (test.mode != kTestNone && row0 < segment.row_count) ? evaluate8(segment, test, row0) : 0u;
+        const uint32_t mask = Rows::mask8(state, row0);
         packed[t] |= mask << (8 * it);
         counts += static_cast<uint32_t>(__popc(mask)) << (16 * t);
       }
@@ -871,7 +928,9 @@ struct FilteredScanParams {
   uint32_t null_row_matches;          // 1: the predicate is IS NULL — a NULL_ROW_ID (outer join) is a NULL value and matches
 };
 
-__global__ void __launch_bounds__(kScanThreads) filtered_scan_kernel(const FilteredScanParams params) {
+template <typename Rows>
+__global__ void __launch_bounds__(kScanThreads) filtered_scan_kernel(const FilteredScanParams params,
+                                                                     const typename Rows::Extra extra) {
   __shared__ hyb_row_id s_rows[kFilteredTileRows];
   __shared__ uint32_t s_warp_totals[kScanWarps];
   __shared__ uint32_t s_tile;
@@ -895,9 +954,7 @@ __global__ void __launch_bounds__(kScanThreads) filtered_scan_kernel(const Filte
       if (index < params.input_count) {
         rows[j] = params.input[index];
         if (rows[j].chunk_id != HYB_INVALID_CHUNK_ID) {
-          const DevSegment& segment = params.segments[rows[j].chunk_id];
-          const ChunkTest& test = params.tests[rows[j].chunk_id];
-          if (evaluate1(segment, test, rows[j].chunk_offset)) mask |= 1u << j;
+          if (Rows::test1(params.segments, params.tests, extra, rows[j].chunk_id, rows[j].chunk_offset)) mask |= 1u << j;
         } else if (params.null_row_matches) {  // NULL_ROW_ID (outer join): the value is NULL; only IS NULL holds
           mask |= 1u << j;
         }
@@ -1097,6 +1154,147 @@ static uint64_t column_bytes_per_launch(const Table* table, uint32_t column_id) 
   return bytes;
 }
 
+// The two-pass pipeline over params.tile_count (> 0) tiles: match bits and tile counts, their prefix, the expansion.
+template <typename Rows>
+static int launch_two_pass(hyb_context* context, const ScanParams& params, const typename Rows::Extra& extra) {
+  const uint32_t tile_count = params.tile_count;
+  uint32_t* masks = nullptr;
+  uint32_t* tile_counts = nullptr;
+  unsigned long long* tile_bases = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(uint32_t) * size_t{tile_count} * kScanThreads, reinterpret_cast<void**>(&masks)));
+  HYB_TRY(device_alloc(context, sizeof(uint32_t) * size_t{tile_count}, reinterpret_cast<void**>(&tile_counts)));
+  HYB_TRY(device_alloc(context, sizeof(unsigned long long) * (size_t{tile_count} + 1), reinterpret_cast<void**>(&tile_bases)));
+  int mask_blocks = 1, expand_blocks = 1;
+  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&mask_blocks, scan_mask_kernel<Rows>, kScanThreads, 0));
+  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&expand_blocks, scan_expand_kernel, kScanThreads, 0));
+  scan_mask_kernel<Rows><<<std::min<uint32_t>(tile_count, context->sm_count * std::max(mask_blocks, 1)), kScanThreads, 0,
+                           context->stream>>>(params, masks, tile_counts, extra);
+  scan_bases_kernel<<<1, 1024, 0, context->stream>>>(tile_counts, tile_count, tile_bases);
+  scan_expand_kernel<<<std::min<uint32_t>(tile_count, context->sm_count * std::max(expand_blocks, 1)), kScanThreads, 0,
+                       context->stream>>>(params, masks, tile_bases);
+  device_free(context, masks);
+  device_free(context, tile_counts);
+  device_free(context, tile_bases);
+  return HYB_OK;
+}
+
+// Input = a previous operator's PosList on the same table: gather, test and emit the referenced RowIDs in input order.
+// null_row_matches: a NULL_ROW_ID (outer join) satisfies the predicate (IS NULL only).
+template <typename Rows>
+static int launch_filtered(hyb_context* context, const PosList* filter, const DevSegment* column_segments,
+                           const ChunkTest* tests, const typename Rows::Extra& extra, bool null_row_matches,
+                           PosList* result, uint64_t* out_input_rows) {
+  const uint32_t chunk_count = result->chunk_count;
+  HYB_CUDA(cudaStreamSynchronize(context->stream));
+  uint64_t input_count = 0;
+  HYB_CUDA(cudaMemcpy(&input_count, filter->d_chunk_end + filter->chunk_count, sizeof(uint64_t),
+                      cudaMemcpyDeviceToHost));
+  if (input_count == ~uint64_t{0}) input_count = 0;
+  *out_input_rows = input_count;
+  result->capacity = input_count;
+  void* out = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * std::max<uint64_t>(input_count, 1), &out));
+  result->d_row_ids = static_cast<hyb_row_id*>(out);
+  const uint32_t tile_count = static_cast<uint32_t>((input_count + kFilteredTileRows - 1) / kFilteredTileRows);
+  void* status = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{tile_count} + 2), &status));
+  HYB_CUDA(cudaMemsetAsync(status, 0, sizeof(uint64_t) * (size_t{tile_count} + 2), context->stream));
+  auto* total = static_cast<unsigned long long*>(status) + tile_count + 1;
+  timing_kernel_begin(context);
+  if (tile_count > 0) {
+    FilteredScanParams params{};
+    params.segments = column_segments;
+    params.tests = tests;
+    params.input = filter->d_row_ids;
+    params.input_count = input_count;
+    params.chunk_count = chunk_count;
+    params.tile_count = tile_count;
+    params.tile_status = static_cast<unsigned long long*>(status);
+    params.ticket = reinterpret_cast<uint32_t*>(static_cast<unsigned long long*>(status) + tile_count);
+    params.out = result->d_row_ids;
+    params.out_total = total;
+    params.null_row_matches = null_row_matches;
+    int blocks_per_sm = 0;
+    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, filtered_scan_kernel<Rows>, kScanThreads, 0));
+    const uint32_t grid = std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1));
+    filtered_scan_kernel<Rows><<<grid, kScanThreads, 0, context->stream>>>(params, extra);
+    HYB_CUDA(cudaGetLastError());
+  }
+  timing_kernel_end(context);
+  if (filter->ascending) {
+    pos_list_chunk_ends_kernel<<<(chunk_count + 1 + 127) / 128, 128, 0, context->stream>>>(
+        result->d_row_ids, total, chunk_count, reinterpret_cast<unsigned long long*>(result->d_chunk_end));
+  } else {
+    // input in another order than the table's (a join's output, abstract_dereferenced_column_table_scan_impl.cpp:49-86):
+    // the matches keep the input order and form ONE list
+    result->chunk_count = 1;
+    result->ascending = false;
+    result->may_hold_null_rows = filter->may_hold_null_rows && null_row_matches;
+    pos_list_chunk_ends_kernel<<<1, 128, 0, context->stream>>>(result->d_row_ids, total, 0u,
+                                                               reinterpret_cast<unsigned long long*>(result->d_chunk_end));
+    HYB_CUDA(cudaMemcpyAsync(result->d_chunk_end + 1, result->d_chunk_end, sizeof(uint64_t), cudaMemcpyDeviceToDevice, context->stream));
+  }
+  HYB_CUDA(cudaGetLastError());
+  device_free(context, status);
+  return HYB_OK;
+}
+
+// Per-chunk PairTests of a column-vs-column predicate, built on the host from the segment descriptors (ColumnVsColumn-
+// TableScanImpl::scan_chunk, column_vs_column_table_scan_impl.cpp). String pairs: the caller's right_in_left words are
+// uploaded once and every chunk points at its slice.
+static int prepare_pair_tests(hyb_context* context, const Table* table, const hyb_column_scan_predicate* predicate,
+                              PairCompare compare, DeviceScratch& scratch, PairTest** out_tests, uint64_t* out_words) {
+  const uint32_t chunk_count = table->chunk_count();
+  const bool strings = table->column_types[predicate->left_column_id] == HYB_TYPE_STRING;
+  std::vector<PairTest> host(chunk_count);
+  std::vector<uint64_t> first_word(chunk_count, 0);
+  uint64_t words = 0;
+  for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+    const DevSegment& left = table->segments[size_t{chunk} * table->column_count + predicate->left_column_id];
+    const DevSegment& right = table->segments[size_t{chunk} * table->column_count + predicate->right_column_id];
+    PairTest& test = host[chunk];
+    test = PairTest{};
+    test.mode = kPairNone;
+    test.condition = predicate->condition;
+    test.compare = compare;
+    if (strings) {
+      HYB_CHECK(left.encoding == HYB_ENC_DICTIONARY && right.encoding == HYB_ENC_DICTIONARY, HYB_ERR_INVALID,
+                "string column-vs-column scans need dictionary segments");
+      HYB_CHECK(left.dict_size < (1u << 31) && right.dict_size < (1u << 31), HYB_ERR_UNSUPPORTED,
+                "column-vs-column scans need dictionaries of fewer than 2^31 entries");
+      first_word[chunk] = words;
+      words += right.dict_size;
+    }
+    const bool all_null = (left.encoding == HYB_ENC_DICTIONARY && left.dict_size == 0) ||
+                          (right.encoding == HYB_ENC_DICTIONARY && right.dict_size == 0);
+    if (left.row_count == 0 || all_null) continue;
+    test.mode = strings ? kPairStringIds : kPairDecoded;
+  }
+  *out_words = words;
+  uint32_t* d_words = nullptr;
+  if (strings && words > 0) {
+    HYB_TRY(scratch.alloc_array(words, &d_words));
+    // pageable source: the copy is staged before cudaMemcpyAsync returns
+    HYB_CUDA(cudaMemcpyAsync(d_words, predicate->right_in_left, sizeof(uint32_t) * words, cudaMemcpyHostToDevice,
+                             context->stream));
+  }
+  for (uint32_t chunk = 0; chunk < chunk_count && d_words; ++chunk) host[chunk].right_in_left = d_words + first_word[chunk];
+  HYB_TRY(scratch.alloc_array(chunk_count, out_tests));
+  if (chunk_count) {
+    HYB_CUDA(cudaMemcpyAsync(*out_tests, host.data(), sizeof(PairTest) * chunk_count, cudaMemcpyHostToDevice,
+                             context->stream));
+  }
+  return HYB_OK;
+}
+
+// The common type of std::less<void> and friends on two numeric column types (C++'s usual arithmetic conversions).
+static PairCompare pair_compare(int32_t left_type, int32_t right_type) {
+  const auto floating = [](int32_t type) { return type == HYB_TYPE_FLOAT32 || type == HYB_TYPE_FLOAT64; };
+  if (left_type == HYB_TYPE_FLOAT64 || right_type == HYB_TYPE_FLOAT64) return kCompareDouble;
+  if (floating(left_type) || floating(right_type)) return kCompareFloat;
+  return kCompareInt64;
+}
+
 }  // namespace hyb
 
 using namespace hyb;
@@ -1182,23 +1380,7 @@ int hyb_table_scan(hyb_context* context, hyb_table_t table_handle, const hyb_sca
       }
       timing_kernel_begin(context);
       if (context->options.scan_two_pass) {
-        uint32_t* masks = nullptr;
-        uint32_t* tile_counts = nullptr;
-        unsigned long long* tile_bases = nullptr;
-        HYB_TRY(device_alloc(context, sizeof(uint32_t) * size_t{tile_count} * kScanThreads, reinterpret_cast<void**>(&masks)));
-        HYB_TRY(device_alloc(context, sizeof(uint32_t) * size_t{tile_count}, reinterpret_cast<void**>(&tile_counts)));
-        HYB_TRY(device_alloc(context, sizeof(unsigned long long) * (size_t{tile_count} + 1), reinterpret_cast<void**>(&tile_bases)));
-        int mask_blocks = 1, expand_blocks = 1;
-        HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&mask_blocks, scan_mask_kernel, kScanThreads, 0));
-        HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&expand_blocks, scan_expand_kernel, kScanThreads, 0));
-        scan_mask_kernel<<<std::min<uint32_t>(tile_count, context->sm_count * std::max(mask_blocks, 1)), kScanThreads, 0,
-                           context->stream>>>(params, masks, tile_counts);
-        scan_bases_kernel<<<1, 1024, 0, context->stream>>>(tile_counts, tile_count, tile_bases);
-        scan_expand_kernel<<<std::min<uint32_t>(tile_count, context->sm_count * std::max(expand_blocks, 1)), kScanThreads, 0,
-                             context->stream>>>(params, masks, tile_bases);
-        device_free(context, masks);
-        device_free(context, tile_counts);
-        device_free(context, tile_bases);
+        HYB_TRY(launch_two_pass<ColumnRows>(context, params, ColumnRows::Extra{}));
         launches = 4;
       } else if (bulk) {
         const uint32_t stage_bytes = kScanTileRows * stream_width;
@@ -1224,63 +1406,109 @@ int hyb_table_scan(hyb_context* context, hyb_table_t table_handle, const hyb_sca
       timing_kernel_end(context);
     }
   } else {
-    // Input = a previous scan's output on the same table.
-    HYB_CUDA(cudaStreamSynchronize(context->stream));
-    uint64_t input_count = 0;
-    HYB_CUDA(cudaMemcpy(&input_count, filter->d_chunk_end + filter->chunk_count, sizeof(uint64_t),
-                        cudaMemcpyDeviceToHost));
-    if (input_count == ~uint64_t{0}) input_count = 0;
-    input_rows = input_count;
-    input_bytes = input_count * sizeof(hyb_row_id);
-    result->capacity = input_count;
-    void* out = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * std::max<uint64_t>(input_count, 1), &out));
-    result->d_row_ids = static_cast<hyb_row_id*>(out);
-    const uint32_t tile_count = static_cast<uint32_t>((input_count + kFilteredTileRows - 1) / kFilteredTileRows);
-    void* status = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{tile_count} + 2), &status));
-    HYB_CUDA(cudaMemsetAsync(status, 0, sizeof(uint64_t) * (size_t{tile_count} + 2), context->stream));
-    auto* total = static_cast<unsigned long long*>(status) + tile_count + 1;
-    timing_kernel_begin(context);
-    if (tile_count > 0) {
-      FilteredScanParams params{};
-      params.segments = column_segments;
-      params.tests = tests;
-      params.input = filter->d_row_ids;
-      params.input_count = input_count;
-      params.chunk_count = chunk_count;
-      params.tile_count = tile_count;
-      params.tile_status = static_cast<unsigned long long*>(status);
-      params.ticket = reinterpret_cast<uint32_t*>(static_cast<unsigned long long*>(status) + tile_count);
-      params.out = result->d_row_ids;
-      params.out_total = total;
-      params.null_row_matches = predicate->condition == HYB_PRED_IS_NULL;
-      int blocks_per_sm = 0;
-      HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, filtered_scan_kernel, kScanThreads, 0));
-      const uint32_t grid = std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1));
-      filtered_scan_kernel<<<grid, kScanThreads, 0, context->stream>>>(params);
-      HYB_CUDA(cudaGetLastError());
-    }
-    timing_kernel_end(context);
-    if (filter->ascending) {
-      pos_list_chunk_ends_kernel<<<(chunk_count + 1 + 127) / 128, 128, 0, context->stream>>>(
-          result->d_row_ids, total, chunk_count, reinterpret_cast<unsigned long long*>(result->d_chunk_end));
-    } else {
-      // input in another order than the table's (a join's output, abstract_dereferenced_column_table_scan_impl.cpp:49-86):
-      // the matches keep the input order and form ONE list
-      result->chunk_count = 1;
-      result->ascending = false;
-      result->may_hold_null_rows = filter->may_hold_null_rows && predicate->condition == HYB_PRED_IS_NULL;
-      pos_list_chunk_ends_kernel<<<1, 128, 0, context->stream>>>(result->d_row_ids, total, 0u,
-                                                                 reinterpret_cast<unsigned long long*>(result->d_chunk_end));
-      HYB_CUDA(cudaMemcpyAsync(result->d_chunk_end + 1, result->d_chunk_end, sizeof(uint64_t), cudaMemcpyDeviceToDevice, context->stream));
-    }
-    HYB_CUDA(cudaGetLastError());
-    device_free(context, status);
+    HYB_TRY(launch_filtered<ColumnRows>(context, filter, column_segments, tests, ColumnRows::Extra{},
+                                        predicate->condition == HYB_PRED_IS_NULL, result.get(), &input_rows));
+    input_bytes = input_rows * sizeof(hyb_row_id);
     launches = 3;
   }
   device_free(context, tests);
   device_free(context, bounds_scratch);
+  timing_end(context, launches, input_bytes, input_rows, 0);
+  timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
+
+  const auto handle = context->next_handle++;
+  context->pos_lists.emplace(handle, std::move(result));
+  *out_pos_list = handle;
+  return HYB_OK;
+}
+
+int hyb_table_scan_columns(hyb_context* context, hyb_table_t table_handle, const hyb_column_scan_predicate* predicate,
+                           hyb_pos_list_t input_filter, hyb_pos_list_t* out_pos_list) {
+  HYB_CHECK(context && predicate && out_pos_list, HYB_ERR_INVALID, "NULL argument");
+  *out_pos_list = 0;
+  DeviceGuard guard(context->device);
+  std::lock_guard<std::mutex> lock(context->mutex);
+  auto* table = find_table(context, table_handle);
+  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  PosList* filter = nullptr;
+  if (input_filter) {
+    filter = find_pos_list(context, input_filter);
+    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
+    HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
+  }
+  const int32_t condition = predicate->condition;
+  HYB_CHECK(!is_like_condition(condition), HYB_ERR_UNSUPPORTED, "column-vs-column LIKE is not on the GPU path");
+  HYB_CHECK(condition >= HYB_PRED_EQUALS && condition <= HYB_PRED_GREATER_THAN_EQUALS, HYB_ERR_INVALID,
+            "column-vs-column scans take =, !=, <, <=, >, >= (condition " + std::to_string(condition) + ")");
+  HYB_CHECK(predicate->left_column_id < table->column_count && predicate->right_column_id < table->column_count,
+            HYB_ERR_INVALID, "column-vs-column scan column out of range");
+  HYB_CHECK(predicate->reserved == 0, HYB_ERR_INVALID, "hyb_column_scan_predicate.reserved must be 0");
+  const int32_t left_type = table->column_types[predicate->left_column_id];
+  const int32_t right_type = table->column_types[predicate->right_column_id];
+  const bool strings = left_type == HYB_TYPE_STRING;
+  // column_vs_column_table_scan_impl.cpp: Fail("Trying to compare strings and non-strings")
+  HYB_CHECK(strings == (right_type == HYB_TYPE_STRING), HYB_ERR_INVALID, "Trying to compare strings and non-strings");
+  HYB_CHECK(!strings || predicate->right_in_left, HYB_ERR_INVALID,
+            "string column-vs-column scans need the host-built right_in_left words (hyb_dictionary_translate)");
+  HYB_TRY(sync_table_descriptors(context, table));
+
+  timing_begin(context);
+  DeviceScratch scratch(context);
+  PairTest* tests = nullptr;
+  uint64_t translation_words = 0;
+  HYB_TRY(prepare_pair_tests(context, table, predicate, strings ? kCompareInt64 : pair_compare(left_type, right_type),
+                             scratch, &tests, &translation_words));
+  const uint32_t chunk_count = table->chunk_count();
+  auto result = std::make_unique<PosList>();
+  result->table = table_handle;
+  result->chunk_count = chunk_count;
+  result->stream = context->stream;
+  result->owner = context;
+  const DevSegment* left_segments = table->d_segments + size_t{predicate->left_column_id} * chunk_count;
+  const PairRows::Extra extra{table->d_segments + size_t{predicate->right_column_id} * chunk_count, tests};
+  uint32_t launches = 1;
+  uint64_t input_rows = 0, input_bytes = sizeof(uint32_t) * translation_words;
+
+  void* chunk_end = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
+  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
+
+  if (!filter) {
+    // Column pairs only have the two-pass pipeline: scan_two_pass = 0 and scan_bulk select one-column kernels only.
+    if (context->options.trace && (!context->options.scan_two_pass || context->options.scan_bulk)) {
+      std::fprintf(stderr, "[hyb] hyb_table_scan_columns: two-pass pipeline (column pairs have no single-pass or bulk kernel)\n");
+    }
+    const uint2* tile_map = nullptr;
+    uint32_t tile_count = 0;
+    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
+    input_rows = table->row_count();
+    input_bytes += column_bytes_per_launch(table, predicate->left_column_id) +
+                   column_bytes_per_launch(table, predicate->right_column_id);
+    result->capacity = table->row_count();
+    void* out = nullptr;
+    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
+    result->d_row_ids = static_cast<hyb_row_id*>(out);
+    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
+    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
+    timing_kernel_begin(context);
+    if (tile_count > 0) {
+      ScanParams params{};
+      params.segments = left_segments;
+      params.tile_map = tile_map;
+      params.chunk_count = chunk_count;
+      params.tile_count = tile_count;
+      params.out = result->d_row_ids;
+      params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
+      HYB_TRY(launch_two_pass<PairRows>(context, params, extra));
+      launches = 4;
+    }
+    timing_kernel_end(context);
+    HYB_CUDA(cudaGetLastError());
+  } else {
+    HYB_TRY(launch_filtered<PairRows>(context, filter, left_segments, nullptr, extra, false, result.get(), &input_rows));
+    input_bytes += input_rows * sizeof(hyb_row_id);
+    launches = 3;
+  }
   timing_end(context, launches, input_bytes, input_rows, 0);
   timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
 

@@ -31,6 +31,37 @@ class Predicate:
     upper: object = None
 
 
+@dataclass
+class ColumnComparison:
+    """left column <condition> right column — the arguments of ColumnVsColumnTableScanImpl; condition is one of
+    PRED_EQUALS .. PRED_GREATER_THAN_EQUALS."""
+
+    left_column_id: int
+    condition: int
+    right_column_id: int
+
+
+def build_column_scan_predicate(table: Table, comparison: ColumnComparison, right_in_left: np.ndarray | None = None,
+                                ) -> tuple[capi.ColumnScanPredicate, object]:
+    """The C struct plus an object that must stay alive while it is in use. String pairs get the translation of the
+    right dictionaries into the left ones (Table.string_column_translation) unless `right_in_left` is given."""
+    struct = capi.ColumnScanPredicate()
+    struct.left_column_id = comparison.left_column_id
+    struct.condition = comparison.condition
+    struct.right_column_id = comparison.right_column_id
+    keepalive = None
+    definitions = table.column_definitions
+    strings = all(column < len(definitions) and definitions[column].data_type == capi.TYPE_STRING
+                  for column in (comparison.left_column_id, comparison.right_column_id))
+    if right_in_left is None and strings:
+        right_in_left = table.string_column_translation(comparison.left_column_id, comparison.right_column_id)
+    if right_in_left is not None:
+        keepalive = np.zeros(max(len(right_in_left), 1), dtype=np.uint32)  # never NULL, even without dictionary entries
+        keepalive[: len(right_in_left)] = right_in_left
+        struct.right_in_left = keepalive.ctypes.data
+    return struct, keepalive
+
+
 def _set_value(target: capi.Value, data_type: int, value) -> None:
     if value is None:
         return
@@ -320,6 +351,18 @@ class DeviceContext:
         handle = C.c_uint64()
         check(self.lib.hyb_table_scan(self.ptr, table.handle, C.byref(struct),
                                       input_filter.handle if input_filter else 0, C.byref(handle)))
+        del keepalive
+        return DevicePosList(self, handle.value)
+
+    def table_scan_columns(self, table: DeviceTable, comparison: ColumnComparison,
+                           input_filter: DevicePosList | None = None, right_in_left: np.ndarray | None = None,
+                           ) -> DevicePosList:
+        """hyb_table_scan_columns: `left <condition> right` per row. String pairs build the right-in-left translation of
+        the host table's dictionaries unless `right_in_left` is given (e.g. NativeBinaryTable.column_translation)."""
+        struct, keepalive = build_column_scan_predicate(table.host_table, comparison, right_in_left)
+        handle = C.c_uint64()
+        check(self.lib.hyb_table_scan_columns(self.ptr, table.handle, C.byref(struct),
+                                              input_filter.handle if input_filter else 0, C.byref(handle)))
         del keepalive
         return DevicePosList(self, handle.value)
 

@@ -372,6 +372,14 @@ class Table:
                  for chunk in self.chunks]
         return np.concatenate(words) if words else np.zeros(0, dtype=np.uint32)
 
+    def string_column_translation(self, left_column_id: int, right_column_id: int) -> np.ndarray:
+        """right_in_left of `left <condition> right` on two string columns: per chunk, hyb_dictionary_translate of the
+        right dictionary into the left one's value-ID space, one uint32 word per right dictionary entry, in chunk order."""
+        words = [capi.dictionary_translate(chunk.segments[left_column_id].string_dictionary,
+                                           chunk.segments[right_column_id].string_dictionary)
+                 for chunk in self.chunks]
+        return np.concatenate(words) if words else np.zeros(0, dtype=np.uint32)
+
     def column_values(self, column_id: int) -> tuple[np.ndarray, np.ndarray]:
         """Decoded values and null mask of a whole column (host side)."""
         if not self.chunks:

@@ -263,6 +263,12 @@ int hyb_binary_table_value_id_bounds(const hyb_binary_table* table, uint32_t col
 int hyb_binary_table_like_bitmaps(const hyb_binary_table* table, uint32_t column, const char* pattern, uint64_t pattern_length,
                                   int32_t condition, uint32_t* out_words, uint32_t* inout_word_count);
 
+/* hyb_column_scan_predicate.right_in_left of two string columns of this table: hyb_dictionary_translate of every chunk's
+ * dictionaries, concatenated in chunk order (one word per right dictionary entry). out_words == NULL: only
+ * *inout_count is set, to the number of words needed; otherwise *inout_count must be at least that. */
+int hyb_binary_table_column_translation(const hyb_binary_table* table, uint32_t left_column, uint32_t right_column,
+                                        uint32_t* out_words, uint32_t* inout_count);
+
 /*
  * Arena upload: when the segment buffers of one or more tables live inside a few large host blocks (a pinned
  * MemoryResource arena, cf. src/lib/memory/default_memory_resource.cpp:29-35 and Chunk::migrate, storage/chunk.hpp:119),
@@ -359,6 +365,44 @@ int hyb_like_dictionary_matches(const char* pattern, uint64_t pattern_length, in
  */
 int hyb_table_scan(hyb_context* context, hyb_table_t table, const hyb_scan_predicate* predicate,
                    hyb_pos_list_t input_filter, hyb_pos_list_t* out_pos_list);
+
+/*
+ * <left column> <condition> <right column>: ColumnVsColumnTableScanImpl (column_vs_column_table_scan_impl.cpp) with the
+ * two-iterator loop of AbstractTableScanImpl::_scan_with_iterators (abstract_table_scan_impl.hpp:56-84). condition is one
+ * of HYB_PRED_EQUALS .. HYB_PRED_GREATER_THAN_EQUALS. A row matches iff neither side is NULL and `left <op> right` holds
+ * in the operands' common type (the usual arithmetic conversions of std::less<void> and friends):
+ *   int32/int64 x int32/int64 -> int64;  int x float -> float (the integer rounded to nearest first);  int32 x double,
+ *   float x double -> double;  int64 x double -> double (the int64 rounded);  float x float -> float.
+ * NaN is unequal to everything (so `!=` holds for it); -0.0 equals +0.0. STRING x STRING compares the bytes as
+ * std::string::compare does; STRING x numeric is HYB_ERR_INVALID, as is any condition outside the six (the LIKE
+ * conditions: HYB_ERR_UNSUPPORTED) or a column id out of range. Both ids may name the same column.
+ * STRING pairs never bring strings to the device: right_in_left holds, for every chunk in chunk order, one word per entry
+ * j of the RIGHT segment's dictionary: 2 * lower_bound(left dictionary of that chunk, right[j]) + (found ? 1 : 0). Left
+ * value-ID i is compared as 2 * i + 1, so the two keys order exactly like the strings. Dictionaries must hold fewer than
+ * 2^31 entries (HYB_ERR_UNSUPPORTED otherwise). hyb_dictionary_translate builds one chunk's words,
+ * hyb_binary_table_column_translation all of a parsed binary table's. Numeric pairs pass right_in_left = NULL.
+ * The output and `input_filter` behave exactly as for hyb_table_scan.
+ */
+typedef struct hyb_column_scan_predicate {
+  uint32_t left_column_id;
+  int32_t condition;              /* HYB_PRED_EQUALS .. HYB_PRED_GREATER_THAN_EQUALS */
+  uint32_t right_column_id;
+  uint32_t reserved;              /* 0 */
+  const uint32_t* right_in_left;  /* STRING pairs only (see above); NULL for numeric pairs */
+} hyb_column_scan_predicate;
+int hyb_table_scan_columns(hyb_context* context, hyb_table_t table, const hyb_column_scan_predicate* predicate,
+                           hyb_pos_list_t input_filter, hyb_pos_list_t* out_pos_list);
+
+/*
+ * right_in_left of one chunk (host only, no GPU): both dictionaries sorted and unique, entry i = chars[offsets[i] ..
+ * offsets[i + 1]) (chars may be NULL when every entry is empty). out_words receives right_count words,
+ * out_words[j] = 2 * lower_bound(left, right[j]) + (right[j] is in left ? 1 : 0), by bytewise comparison (unsigned
+ * chars; a proper prefix sorts first). One merge of the two dictionaries. HYB_ERR_UNSUPPORTED: a dictionary of 2^31
+ * entries or more.
+ */
+int hyb_dictionary_translate(const char* left_chars, const uint64_t* left_offsets, uint32_t left_count,
+                             const char* right_chars, const uint64_t* right_offsets, uint32_t right_count,
+                             uint32_t* out_words);
 
 /* Total matches and per-chunk boundaries: out_chunk_offsets has chunk_count + 1 entries; chunk c's RowIDs are
  * [out_chunk_offsets[c], out_chunk_offsets[c+1]) of the flat list. Either pointer may be NULL. */

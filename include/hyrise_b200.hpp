@@ -145,6 +145,15 @@ class BinaryTable {
     check(hyb_binary_table_like_bitmaps(_table, column, pattern.data(), pattern.size(), condition, bitmaps.data(), &words));
     return bitmaps;
   }
+  // hyb_column_scan_predicate.right_in_left of `left <condition> right` on two string columns: every chunk's right
+  // dictionary translated into its left dictionary's value-ID space (hyb_dictionary_translate)
+  std::vector<uint32_t> column_translation(uint32_t left_column, uint32_t right_column) const {
+    uint32_t words = 0;
+    check(hyb_binary_table_column_translation(_table, left_column, right_column, nullptr, &words));
+    std::vector<uint32_t> translation(std::max<uint32_t>(words, 1));
+    check(hyb_binary_table_column_translation(_table, left_column, right_column, translation.data(), &words));
+    return translation;
+  }
 
  private:
   hyb_binary_table* _table = nullptr;
@@ -363,23 +372,50 @@ struct ScanPredicate {
   }
 };
 
+// left column <condition> right column (ColumnVsColumnTableScanImpl): condition is one of Equals .. GreaterThanEquals.
+// String pairs carry the per-chunk translation of the right dictionaries into the left ones
+// (BinaryTable::column_translation, hyb_dictionary_translate); numeric pairs leave it empty.
+struct ColumnComparison {
+  ColumnID left_column_id;
+  PredicateCondition condition;
+  ColumnID right_column_id;
+  std::vector<uint32_t> right_in_left;
+
+  hyb_column_scan_predicate to_abi() const {
+    hyb_column_scan_predicate predicate{};
+    predicate.left_column_id = left_column_id;
+    predicate.condition = static_cast<int32_t>(condition);
+    predicate.right_column_id = right_column_id;
+    predicate.right_in_left = right_in_left.empty() ? nullptr : right_in_left.data();
+    return predicate;
+  }
+};
+
 class TableScan : public Operator<PosListSet> {
  public:
   TableScan(OperatorInput input, ScanPredicate predicate) : _input(std::move(input)), _predicate(std::move(predicate)) {}
+  TableScan(OperatorInput input, ColumnComparison comparison)
+      : _input(std::move(input)), _comparison(std::move(comparison)) {}
 
  protected:
   std::shared_ptr<const PosListSet> _on_execute() override {
-    const auto abi = _predicate.to_abi();
     hyb_context* context = _input.table->context()->get();
     hyb_pos_list_t handle = 0;
-    check(hyb_table_scan(context, _input.table->handle(), &abi, _input.filter_handle(), &handle));
+    if (_comparison) {
+      const auto abi = _comparison->to_abi();
+      check(hyb_table_scan_columns(context, _input.table->handle(), &abi, _input.filter_handle(), &handle));
+    } else {
+      const auto abi = _predicate->to_abi();
+      check(hyb_table_scan(context, _input.table->handle(), &abi, _input.filter_handle(), &handle));
+    }
     check(hyb_last_operator_stats(context, &performance_data));
     return std::make_shared<PosListSet>(_input.table, handle);
   }
 
  private:
   OperatorInput _input;
-  ScanPredicate _predicate;
+  std::optional<ScanPredicate> _predicate;
+  std::optional<ColumnComparison> _comparison;
 };
 
 // operator_join_predicate.hpp:16-44 — JoinHash supports exactly one equality predicate on the device.

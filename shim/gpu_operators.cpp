@@ -104,6 +104,45 @@ bool like_dictionary_bitmaps(const Table& stored, ColumnID column_id, PredicateC
   return true;
 }
 
+// hyb_column_scan_predicate.right_in_left: per chunk, every right dictionary entry as 2 * lower_bound in the left dictionary
+// + (found ? 1 : 0), one merge of the two sorted dictionaries; one word per right entry, chunk after chunk. Only
+// DictionarySegment<pmr_string> / FixedStringDictionarySegment dictionaries (false: the CPU operator runs).
+bool column_translation(const Table& stored, ColumnID left_column_id, ColumnID right_column_id, std::vector<uint32_t>& words) {
+  const auto dictionary_of = [&](const ChunkID chunk_id, const ColumnID column_id) -> std::optional<std::vector<pmr_string>> {
+    const auto segment = stored.get_chunk(chunk_id)->get_segment(column_id);
+    if (const auto dictionary_segment = std::dynamic_pointer_cast<const DictionarySegment<pmr_string>>(segment)) {
+      const auto& dictionary = *dictionary_segment->dictionary();
+      return std::vector<pmr_string>(dictionary.begin(), dictionary.end());
+    }
+    if (const auto fixed_segment = std::dynamic_pointer_cast<const FixedStringDictionarySegment<pmr_string>>(segment)) {
+      const auto& dictionary = *fixed_segment->fixed_string_dictionary();
+      auto entries = std::vector<pmr_string>{};
+      entries.reserve(dictionary.size());
+      for (auto entry = size_t{0}; entry < dictionary.size(); ++entry) {
+        entries.emplace_back(dictionary.get_string_at(entry));
+      }
+      return entries;
+    }
+    return std::nullopt;
+  };
+  for (auto chunk_id = ChunkID{0}; chunk_id < stored.chunk_count(); ++chunk_id) {
+    const auto left = dictionary_of(chunk_id, left_column_id);
+    const auto right = dictionary_of(chunk_id, right_column_id);
+    if (!left || !right || left->size() >= (size_t{1} << 31) || right->size() >= (size_t{1} << 31)) {
+      return false;
+    }
+    auto position = size_t{0};
+    for (const auto& value : *right) {
+      while (position < left->size() && (*left)[position] < value) {
+        ++position;
+      }
+      const auto found = position < left->size() && (*left)[position] == value;
+      words.push_back(static_cast<uint32_t>(2 * position + (found ? 1 : 0)));
+    }
+  }
+  return true;
+}
+
 // PosLists of a device result -> one output chunk of ReferenceSegments per input chunk with matches (table_scan.cpp:199-217).
 std::shared_ptr<const Table> wrap_pos_lists(hyb_context* context, const std::shared_ptr<const Table>& stored, hyb_pos_list_t result) {
   auto chunk_count = uint32_t{0};
@@ -197,6 +236,38 @@ std::shared_ptr<const Table> try_gpu_table_scan(const std::shared_ptr<const Tabl
   const auto status = hyb_table_scan(pool->context(), entry->handle, &predicate, 0, &result);
   if (status == HYB_ERR_UNSUPPORTED) {
     return nullptr;
+  }
+  Assert(status == HYB_OK, hyb_last_error());
+  return wrap_pos_lists(pool->context(), in_table, result);
+}
+
+std::shared_ptr<const Table> try_gpu_column_scan(const std::shared_ptr<const Table>& in_table, ColumnID left_column_id,
+                                                 PredicateCondition condition, ColumnID right_column_id) {
+  auto* pool = gpu_column_pool();
+  if (!pool || in_table->type() != TableType::Data) {
+    return nullptr;  // reference-table inputs: as in try_gpu_table_scan
+  }
+  const auto* entry = pool->find(in_table);
+  if (!entry) {
+    return nullptr;
+  }
+  auto predicate = hyb_column_scan_predicate{};
+  predicate.left_column_id = left_column_id;
+  predicate.condition = static_cast<int32_t>(condition);  // PredicateCondition and hyb_predicate_condition share values
+  predicate.right_column_id = right_column_id;
+  auto words = std::vector<uint32_t>{};
+  if (in_table->column_data_type(left_column_id) == DataType::String &&
+      in_table->column_data_type(right_column_id) == DataType::String) {
+    if (!column_translation(*in_table, left_column_id, right_column_id, words)) {
+      return nullptr;
+    }
+    words.push_back(0);  // never a NULL pointer, even when no chunk has a dictionary entry
+    predicate.right_in_left = words.data();
+  }
+  auto result = hyb_pos_list_t{};
+  const auto status = hyb_table_scan_columns(pool->context(), entry->handle, &predicate, 0, &result);
+  if (status == HYB_ERR_UNSUPPORTED) {
+    return nullptr;  // LIKE between two columns: the reference operator reports it itself
   }
   Assert(status == HYB_OK, hyb_last_error());
   return wrap_pos_lists(pool->context(), in_table, result);

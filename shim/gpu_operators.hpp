@@ -26,6 +26,11 @@ std::shared_ptr<const Table> try_gpu_table_scan(const std::shared_ptr<const Tabl
                                                 PredicateCondition condition, const AllTypeVariant& value,
                                                 const std::optional<AllTypeVariant>& value2);
 
+// TableScan::_on_execute when create_impl would pick a ColumnVsColumnTableScanImpl (table_scan.cpp:312-452): the single
+// OperatorScanPredicate compares two columns of a stored table. String columns need dictionary segments.
+std::shared_ptr<const Table> try_gpu_column_scan(const std::shared_ptr<const Table>& in_table, ColumnID left_column_id,
+                                                 PredicateCondition condition, ColumnID right_column_id);
+
 // JoinHash::_on_execute (join_hash.cpp:116-225), after the build/probe side selection and the radix-bit calculation.
 std::shared_ptr<const Table> try_gpu_join_hash(const std::shared_ptr<const Table>& build_table,
                                                const std::shared_ptr<const Table>& probe_table, ColumnID build_column_id,
