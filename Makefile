@@ -14,8 +14,9 @@ TPCH_LIB  := hyrise_b200/lib/libhyb_tpch.so
 
 COLUMN_SCAN_ORACLE := build/libcolumn_scan_oracle.so
 AGGREGATE_DISTINCT_ORACLE := build/libaggregate_distinct_oracle.so
+IN_SCAN_ORACLE := build/libin_scan_oracle.so
 
-all: $(LIB) $(TPCH_LIB) oracle $(COLUMN_SCAN_ORACLE) $(AGGREGATE_DISTINCT_ORACLE)
+all: $(LIB) $(TPCH_LIB) oracle $(COLUMN_SCAN_ORACLE) $(AGGREGATE_DISTINCT_ORACLE) $(IN_SCAN_ORACLE)
 
 build/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p build
@@ -67,6 +68,18 @@ $(AGGREGATE_DISTINCT_ORACLE): tests/cpp/aggregate_distinct_oracle.cpp include/hy
 build/aggregate_distinct_check: tests/cpp/aggregate_distinct_check.cpp include/hyrise_b200.hpp include/hyrise_b200.h $(LIB)
 	@mkdir -p build
 	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/aggregate_distinct_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
+		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
+
+# CPU restatement of the ExpressionEvaluator's IN over a literal list (test infrastructure, tests/in_scan_oracle.py).
+# No -ffast-math: NaN and signed zeros must compare as std::equal_to does.
+$(IN_SCAN_ORACLE): tests/cpp/in_scan_oracle.cpp include/hyrise_b200.h
+	@mkdir -p build
+	$(CXX) -O2 -std=c++17 -fPIC -Wall -Wextra -shared -o $@ tests/cpp/in_scan_oracle.cpp
+
+# [NOT] IN TableScans through the mirror on the GPU (a numeric and a string list).
+build/in_scan_check: tests/cpp/in_scan_check.cpp include/hyrise_b200.hpp include/hyrise_b200.h $(LIB)
+	@mkdir -p build
+	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/in_scan_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
 		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
 
 clean:

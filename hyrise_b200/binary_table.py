@@ -394,6 +394,17 @@ class NativeBinaryTable:
                                                           words.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(count)))
         return words[: count.value]
 
+    def in_bitmaps(self, column: int, condition: int, elements) -> np.ndarray:
+        """hyb_binary_table_in_bitmaps: dictionary_matches of `<string column> [NOT] IN (elements)` (bytes)."""
+        chars, offsets = capi._string_dictionary_arguments(elements)
+        arguments = (self.ptr, column, condition, chars, offsets.ctypes.data_as(C.POINTER(C.c_uint64)), len(offsets) - 1)
+        count = C.c_uint32()
+        capi.check(self.lib.hyb_binary_table_in_bitmaps(*arguments, None, C.byref(count)))
+        words = np.zeros(max(count.value, 1), dtype=np.uint32)
+        capi.check(self.lib.hyb_binary_table_in_bitmaps(*arguments, words.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                                        C.byref(count)))
+        return words[: count.value]
+
     def column_translation(self, left_column: int, right_column: int) -> np.ndarray:
         """hyb_binary_table_column_translation: right_in_left of a column-vs-column scan on two string columns."""
         count = C.c_uint32()

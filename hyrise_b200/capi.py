@@ -107,6 +107,17 @@ class Literal(C.Structure):
     _fields_ = [("data_type", C.c_int32), ("value", Value)]
 
 
+class InPredicate(C.Structure):
+    _fields_ = [
+        ("column_id", C.c_uint32),
+        ("condition", C.c_int32),
+        ("element_count", C.c_uint32),
+        ("has_null_element", C.c_uint32),
+        ("elements", C.POINTER(Literal)),
+        ("dictionary_matches", C.c_void_p),
+    ]
+
+
 class JoinSide(C.Structure):
     _fields_ = [("table", C.c_uint64), ("column_id", C.c_uint32), ("filter", C.c_uint64)]
 
@@ -199,6 +210,12 @@ SYMBOLS = {
     "hyb_dictionary_translate": [C.c_void_p, C.POINTER(_U64), _U32, C.c_void_p, C.POINTER(_U64), _U32, C.POINTER(_U32)],
     "hyb_table_scan": [_CTX, _U64, C.POINTER(ScanPredicate), _U64, C.POINTER(_U64)],
     "hyb_table_scan_columns": [_CTX, _U64, C.POINTER(ColumnScanPredicate), _U64, C.POINTER(_U64)],
+    "hyb_table_scan_in": [_CTX, _U64, C.POINTER(InPredicate), _U64, C.POINTER(_U64)],
+    "hyb_in_dictionary_matches": [_I32, C.c_void_p, C.POINTER(_U64), _U32, C.c_void_p, C.POINTER(_U64), _U32,
+                                  C.POINTER(_U32), C.POINTER(_U32)],
+    "hyb_binary_table_in_bitmaps": [C.c_void_p, _U32, _I32, C.c_void_p, C.POINTER(_U64), _U32, C.POINTER(_U32),
+                                    C.POINTER(_U32)],
+    "hyb_in_list_normalize": [_I32, C.POINTER(Literal), _U32, C.POINTER(Value), C.POINTER(_U32)],
     "hyb_pos_list_info": [_CTX, _U64, C.POINTER(_U64), C.POINTER(_U32)],
     "hyb_pos_list_chunk_offsets": [_CTX, _U64, _P],
     "hyb_pos_list_copy": [_CTX, _U64, _U64, _U64, _P],
@@ -282,6 +299,54 @@ def dictionary_translate(left_entries, right_entries) -> "np.ndarray":
                                                   right_offsets.ctypes.data_as(C.POINTER(C.c_uint64)), count,
                                                   words.ctypes.data_as(C.POINTER(C.c_uint32))))
     return words[:count]
+
+
+def in_dictionary_matches(condition: int, elements, entries) -> "np.ndarray":
+    """hyb_in_dictionary_matches: membership of every entry of one string dictionary (a sequence of bytes) in the list
+    `elements` (bytes, any order, repeats allowed) as ceil(len / 32) uint32 words, entry i = bit i & 31 of word i >> 5;
+    NOT IN is already inverted. Host only."""
+    import numpy as np
+
+    element_chars, element_offsets = _string_dictionary_arguments(elements)
+    chars, offsets = _string_dictionary_arguments(entries)
+    count = len(offsets) - 1
+    words = np.zeros(max((count + 31) // 32, 1), dtype=np.uint32)
+    check(load_library().hyb_in_dictionary_matches(condition, element_chars,
+                                                   element_offsets.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                   len(element_offsets) - 1, chars,
+                                                   offsets.ctypes.data_as(C.POINTER(C.c_uint64)), count,
+                                                   words.ctypes.data_as(C.POINTER(C.c_uint32)), None))
+    return words[: (count + 31) // 32]
+
+
+def literal_array(literals) -> "C.Array":
+    """A ctypes array of hyb_literal from (data_type, value) pairs of numeric types (at least one slot)."""
+    array = (Literal * max(len(literals), 1))()
+    for index, (data_type, value) in enumerate(literals):
+        array[index].data_type = data_type
+        if data_type == TYPE_INT32:
+            array[index].value.i32 = int(value)
+        elif data_type == TYPE_INT64:
+            array[index].value.i64 = int(value)
+        elif data_type == TYPE_FLOAT32:
+            array[index].value.f32 = float(value)
+        elif data_type == TYPE_FLOAT64:
+            array[index].value.f64 = float(value)
+    return array
+
+
+def in_list_normalize(column_type: int, literals) -> list:
+    """hyb_in_list_normalize: the numeric list `literals` ((data_type, value) pairs) as the sorted, disjoint closed
+    intervals [(lo, hi), ...] of `column_type` values it matches; Python ints for integer columns, floats otherwise
+    (float32 bounds exactly representable). Host only."""
+    elements = literal_array(literals)
+    count = C.c_uint32(0)
+    lib = load_library()
+    check(lib.hyb_in_list_normalize(column_type, elements, len(literals), None, C.byref(count)))
+    bounds = (Value * max(2 * count.value, 1))()
+    check(lib.hyb_in_list_normalize(column_type, elements, len(literals), bounds, C.byref(count)))
+    member = {TYPE_INT32: "i32", TYPE_INT64: "i64", TYPE_FLOAT32: "f32", TYPE_FLOAT64: "f64"}[column_type]
+    return [(getattr(bounds[2 * i], member), getattr(bounds[2 * i + 1], member)) for i in range(count.value)]
 
 
 IPC_HANDLE_BYTES = 64

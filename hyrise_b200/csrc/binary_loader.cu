@@ -549,6 +549,33 @@ int hyb_binary_table_like_bitmaps(const hyb_binary_table* table, uint32_t column
   return HYB_OK;
 }
 
+int hyb_binary_table_in_bitmaps(const hyb_binary_table* table, uint32_t column, int32_t condition, const char* element_chars,
+                                const uint64_t* element_offsets, uint32_t element_count, uint32_t* out_words,
+                                uint32_t* inout_word_count) {
+  HYB_CHECK(table && inout_word_count, HYB_ERR_INVALID, "NULL argument");
+  const size_t columns = table->column_types.size();
+  HYB_CHECK(column < columns && table->column_types[column] == HYB_TYPE_STRING, HYB_ERR_INVALID, "not a string column");
+  std::vector<LikeDictionary> dictionaries(table->chunk_rows.size());
+  uint64_t words = 0;
+  for (size_t chunk = 0; chunk < table->chunk_rows.size(); ++chunk) {
+    const auto& dictionary = table->string_dictionaries[chunk * columns + column];
+    const uint32_t size = dictionary.offsets.empty() ? 0 : static_cast<uint32_t>(dictionary.offsets.size() - 1);
+    // chars.data() is NULL for a dictionary that holds only the empty string
+    dictionaries[chunk] = LikeDictionary{dictionary.chars.data(), dictionary.offsets.data(), size};
+    words += (size_t{size} + 31) / 32;
+  }
+  HYB_CHECK(words <= UINT32_MAX, HYB_ERR_INVALID, "bitmap exceeds 2^32 words");
+  if (!out_words) {
+    *inout_word_count = static_cast<uint32_t>(words);
+    return HYB_OK;
+  }
+  HYB_CHECK(*inout_word_count >= words, HYB_ERR_INVALID, "out_words holds fewer words than the bitmaps need");
+  HYB_TRY(in_match_dictionaries(condition, LikeDictionary{element_chars, element_offsets, element_count},
+                                dictionaries.data(), dictionaries.size(), out_words, nullptr));
+  *inout_word_count = static_cast<uint32_t>(words);
+  return HYB_OK;
+}
+
 int hyb_binary_table_column_translation(const hyb_binary_table* table, uint32_t left_column, uint32_t right_column,
                                         uint32_t* out_words, uint32_t* inout_count) {
   HYB_CHECK(table && inout_count, HYB_ERR_INVALID, "NULL argument");

@@ -281,6 +281,11 @@ int like_match_dictionaries(const char* pattern, uint64_t pattern_length, int32_
 // hyb_dictionary_translate (translate.cu): right_in_left of one chunk, right.count words, for two sorted unique
 // dictionaries in the layout above.
 int translate_dictionary(const LikeDictionary& left, const LikeDictionary& right, uint32_t* out_words);
+// hyb_in_dictionary_matches (in_list.cu) over several dictionaries, their bitmaps concatenated in out_words.
+int in_match_dictionaries(int32_t condition, const LikeDictionary& elements, const LikeDictionary* dictionaries,
+                          size_t dictionary_count, uint32_t* out_words, uint64_t* out_match_count);
+// hyb_in_list_normalize (in_list.cu): [lo, hi] pairs in the column type's member of hyb_value.
+int normalize_in_list(int32_t column_type, const hyb_literal* elements, uint32_t count, std::vector<hyb_value>& out_bounds);
 
 // Helpers implemented in context.cu ---------------------------------------------------------------------------------
 class DeviceGuard {
@@ -332,6 +337,10 @@ class DeviceScratch {
     const int status = alloc(sizeof(T) * (count ? count : 1), &block);
     *out = static_cast<T*>(block);
     return status;
+  }
+  // Release a block taken with device_alloc together with this scope's blocks (nullptr: nothing to do).
+  void adopt(void* block) {
+    if (block) _blocks.push_back(block);
   }
   // Hand a block over to a result object (it is no longer released by this scope).
   void* release(void* block) {

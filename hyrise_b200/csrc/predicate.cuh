@@ -12,7 +12,9 @@ enum ChunkTestMode : uint32_t {
   kTestInt = 2,         // typed integer range (ValueSegment<int32/int64>, FrameOfReference)
   kTestFloat = 3,       // typed floating-point range (ValueSegment<float/double>)
   kTestNull = 4,        // IS NULL / IS NOT NULL on a null vector
-  kTestIdSet = 5        // dictionary value-ID set (LIKE): match iff value_id < dict_size and its bit in id_bits is set
+  kTestIdSet = 5,       // dictionary value-ID set (LIKE): match iff value_id < dict_size and its bit in id_bits is set
+  kTestInList = 6,      // [NOT] IN on a Value / FrameOfReference segment: the list's intervals (in_list.cuh)
+  kTestAll = 7          // every row, NULL rows included (NOT IN over a list without a compatible element)
 };
 
 struct ChunkTest {

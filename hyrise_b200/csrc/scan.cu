@@ -20,7 +20,10 @@
 //
 // Column-vs-column predicates (hyb_table_scan_columns, ColumnVsColumnTableScanImpl) run through the same two-pass and
 // position-filtered kernels: scan_mask_kernel and filtered_scan_kernel are templates on the row evaluator (ColumnRows:
-// one column against its ChunkTest; PairRows: two columns against a PairTest, column_pair.cuh).
+// one column against its ChunkTest; PairRows: two columns against a PairTest, column_pair.cuh). `<column> [NOT] IN (...)`
+// (hyb_table_scan_in, the ExpressionEvaluator's _evaluate_in_expression on a literal list) uses them too, with InRows:
+// dictionary chunks scan a value-ID range or set built by in_prepare_kernel (numeric) or from the caller's dictionary
+// bitmaps (strings), Value / FrameOfReference chunks search the list's intervals (in_list.cuh).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -30,6 +33,7 @@
 #include "bulk_copy.cuh"
 #include "column_pair.cuh"
 #include "device_utils.cuh"
+#include "in_list.cuh"
 #include "internal.hpp"
 #include "predicate.cuh"
 
@@ -512,6 +516,49 @@ struct PairRows {  // <left column> <condition> <right column>: the params' segm
     const PairTest& test = extra.tests[chunk];
     if (test.mode == kPairNone) return false;
     return evaluate1_pair(segments[chunk], extra.right_segments[chunk], test, row);
+  }
+};
+
+struct InRows {  // <column> [NOT] IN (<literal>, ...): the chunk's ChunkTest, and the list's intervals for Value / FoR chunks
+  using Extra = InList;
+  struct Chunk {
+    DevSegment segment;
+    ChunkTest test;
+    InList list;
+  };
+  static __device__ __forceinline__ Chunk chunk(const ScanParams& params, const Extra& extra, uint32_t chunk) {
+    return Chunk{params.segments[chunk], params.tests[chunk], extra};
+  }
+  static __device__ __forceinline__ uint32_t mask8(const Chunk& state, uint32_t row0) {
+    if (row0 >= state.segment.row_count) return 0u;
+    switch (state.test.mode) {
+      case kTestIdRange:
+      case kTestIdSet:
+        return evaluate8(state.segment, state.test, row0);
+      case kTestInList:
+        return evaluate8_in(state.segment, state.test, state.list, row0);
+      case kTestAll: {
+        const uint32_t rows = state.segment.row_count - row0;
+        return rows >= 8 ? 0xFFu : ((1u << rows) - 1u);
+      }
+      default:
+        return 0u;
+    }
+  }
+  static __device__ __forceinline__ bool test1(const DevSegment* segments, const ChunkTest* tests, const Extra& extra,
+                                               uint32_t chunk, uint32_t row) {
+    const ChunkTest& test = tests[chunk];
+    switch (test.mode) {
+      case kTestIdRange:
+      case kTestIdSet:
+        return evaluate1(segments[chunk], test, row);
+      case kTestInList:
+        return evaluate1_in(segments[chunk], test, extra, row);
+      case kTestAll:
+        return true;
+      default:
+        return false;
+    }
   }
 };
 
@@ -1019,26 +1066,28 @@ static bool supported_condition(int32_t condition) {
          condition == HYB_PRED_IS_NULL || condition == HYB_PRED_IS_NOT_NULL;
 }
 
-// LIKE: the caller's per-chunk dictionary match bitmaps (ColumnLikeTableScanImpl::_find_matches_in_dictionary,
-// column_like_table_scan_impl.cpp:75-140) become per-chunk tests on the host, which reads the bitmaps anyway. No bit set:
-// kTestNone (the chunk's bytes are skipped); one contiguous run of set bits (every entry, or a prefix pattern on a sorted
-// dictionary): kTestIdRange, as fast as a range scan; anything else: kTestIdSet, and only those chunks' words are uploaded.
-static int prepare_like_tests(hyb_context* context, Table* table, const hyb_scan_predicate* predicate, void* tests,
-                              void** out_bitmap_scratch) {
+// Dictionary match bitmaps of a string column (LIKE: ColumnLikeTableScanImpl::_find_matches_in_dictionary,
+// column_like_table_scan_impl.cpp:75-140; IN: hyb_in_dictionary_matches) become per-chunk tests on the host, which reads
+// the bitmaps anyway. No bit set: kTestNone (the chunk's bytes are skipped); one contiguous run of set bits (every entry,
+// or a prefix pattern on a sorted dictionary): kTestIdRange, as fast as a range scan; anything else: kTestIdSet, and only
+// those chunks' words are uploaded (*out_uploaded_words, optional, counts them).
+static int prepare_bitmap_tests(hyb_context* context, Table* table, uint32_t column_id, const uint32_t* bitmaps, void* tests,
+                                void** out_bitmap_scratch, uint64_t* out_uploaded_words = nullptr) {
   const uint32_t chunk_count = table->chunk_count();
   std::vector<ChunkTest> host(chunk_count);
   std::vector<uint32_t> set_words;
   size_t word = 0;
   for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
-    const DevSegment& segment = table->segments[size_t{chunk} * table->column_count + predicate->column_id];
+    const DevSegment& segment = table->segments[size_t{chunk} * table->column_count + column_id];
     const uint32_t size = segment.dict_size;
-    const uint32_t* bits = predicate->value_id_bounds + word;
+    const uint32_t* bits = bitmaps + word;
     word += (size_t{size} + 31) / 32;
     ChunkTest& test = host[chunk];
     test = ChunkTest{};
     test.mode = kTestNone;
     if (segment.row_count == 0) continue;
-    HYB_CHECK(segment.encoding == HYB_ENC_DICTIONARY, HYB_ERR_INVALID, "LIKE needs dictionary-encoded string segments");
+    HYB_CHECK(segment.encoding == HYB_ENC_DICTIONARY, HYB_ERR_INVALID,
+              "dictionary bitmaps need dictionary-encoded string segments");
     uint32_t count = 0, first = 0, last = 0;
     for (uint32_t w = 0; w < (size + 31) / 32; ++w) {
       uint32_t bits_w = bits[w];
@@ -1059,6 +1108,7 @@ static int prepare_like_tests(hyb_context* context, Table* table, const hyb_scan
       set_words.insert(set_words.end(), bits, bits + (size + 31) / 32);
     }
   }
+  if (out_uploaded_words) *out_uploaded_words = set_words.size();
   if (!set_words.empty()) {
     HYB_TRY(device_alloc(context, sizeof(uint32_t) * set_words.size(), out_bitmap_scratch));
     const auto* base = static_cast<const uint32_t*>(*out_bitmap_scratch);
@@ -1096,7 +1146,8 @@ int prepare_chunk_tests(hyb_context* context, Table* table, const hyb_scan_predi
               "LIKE scans need host-computed dictionary match bitmaps in value_id_bounds (hyb_like_dictionary_matches)");
     void* tests = nullptr;
     HYB_TRY(device_alloc(context, sizeof(ChunkTest) * std::max<uint32_t>(chunk_count, 1), &tests));
-    const int status = prepare_like_tests(context, table, predicate, tests, out_bounds_scratch);
+    const int status =
+        prepare_bitmap_tests(context, table, predicate->column_id, predicate->value_id_bounds, tests, out_bounds_scratch);
     if (status != HYB_OK) {
       device_free(context, tests);
       device_free(context, *out_bounds_scratch);
@@ -1293,6 +1344,142 @@ static PairCompare pair_compare(int32_t left_type, int32_t right_type) {
   if (left_type == HYB_TYPE_FLOAT64 || right_type == HYB_TYPE_FLOAT64) return kCompareDouble;
   if (floating(left_type) || floating(right_type)) return kCompareFloat;
   return kCompareInt64;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// [NOT] IN on a numeric column: per-chunk tests from the list's intervals. A dictionary chunk maps every interval [lo, hi]
+// to the value-IDs [lower_bound(lo), upper_bound(hi)) of its device-resident dictionary; the ranges are sorted and
+// disjoint like the intervals, and ranges that touch form one run. No run: kTestNone (IN) or every non-NULL row (NOT IN);
+// one run: kTestIdRange, negated for NOT IN; more: a kTestIdSet bitmap written here (inverted for NOT IN; the NULL id is
+// never set). Value / FrameOfReference chunks search the intervals per row (kTestInList).
+// ---------------------------------------------------------------------------------------------------------------------
+template <typename Conv>
+__device__ void dictionary_id_range(const DevSegment& segment, const InList& list, uint32_t interval, uint32_t& lower,
+                                    uint32_t& upper) {
+  using T = typename Conv::T;
+  const T lo = static_cast<const T*>(list.bounds)[2 * interval];
+  const T hi = static_cast<const T*>(list.bounds)[2 * interval + 1];
+  uint32_t a = 0, b = segment.dict_size;
+  while (a < b) {  // first entry >= lo
+    const uint32_t mid = (a + b) >> 1;
+    if (gather_entry<Conv>(segment, mid) < lo) {
+      a = mid + 1;
+    } else {
+      b = mid;
+    }
+  }
+  lower = a;
+  b = segment.dict_size;
+  while (a < b) {  // first entry > hi; a NaN entry (sorted last) counts as greater
+    const uint32_t mid = (a + b) >> 1;
+    if (gather_entry<Conv>(segment, mid) <= hi) {
+      a = mid + 1;
+    } else {
+      b = mid;
+    }
+  }
+  upper = a;
+}
+
+template <typename Conv>
+__device__ void in_dictionary_test(const DevSegment& segment, const InList& list, bool negate, uint32_t* bits,
+                                   ChunkTest& test) {
+  const uint32_t size = segment.dict_size;
+  uint32_t runs = 0, first_lo = 0, first_hi = 0, last_hi = 0;
+  for (uint32_t i = 0; i < list.interval_count; ++i) {
+    uint32_t a, b;
+    dictionary_id_range<Conv>(segment, list, i, a, b);
+    if (a >= b) continue;
+    if (runs > 0 && a == last_hi) {  // touches the previous run
+      last_hi = b;
+      if (runs == 1) first_hi = b;
+      continue;
+    }
+    if (runs == 0) {
+      first_lo = a;
+      first_hi = b;
+    }
+    ++runs;
+    last_hi = b;
+  }
+  if (runs == 0) {
+    if (negate && size > 0) {  // no entry is in the list: every non-NULL row matches NOT IN
+      test.mode = kTestIdRange;
+      test.id_lo = 0;
+      test.id_span = size;
+    }
+    return;
+  }
+  if (runs == 1) {
+    test.mode = kTestIdRange;
+    test.negate = negate;
+    test.id_lo = first_lo;
+    test.id_span = first_hi - first_lo;
+    return;
+  }
+  const uint32_t words = (size + 31) / 32;
+  for (uint32_t w = 0; w < words; ++w) bits[w] = 0u;
+  for (uint32_t i = 0; i < list.interval_count; ++i) {
+    uint32_t a, b;
+    dictionary_id_range<Conv>(segment, list, i, a, b);
+    for (uint32_t id = a; id < b;) {  // whole words where the range covers them
+      const uint32_t bit = id & 31u, take = min(32u - bit, b - id);
+      bits[id >> 5] |= (take == 32u ? 0xFFFFFFFFu : ((1u << take) - 1u)) << bit;
+      id += take;
+    }
+  }
+  if (negate) {
+    for (uint32_t w = 0; w < words; ++w) bits[w] = ~bits[w];
+    if (size & 31u) bits[words - 1] &= (1u << (size & 31u)) - 1u;
+  }
+  test.mode = kTestIdSet;
+  test.id_bits = bits;
+}
+
+__global__ void in_prepare_kernel(const DevSegment* __restrict__ segments, uint32_t chunk_count, InList list,
+                                  uint32_t negate, const unsigned long long* __restrict__ word_offsets,
+                                  uint32_t* __restrict__ bits, ChunkTest* __restrict__ tests) {
+  const uint32_t chunk = blockIdx.x * blockDim.x + threadIdx.x;
+  if (chunk >= chunk_count) return;
+  const DevSegment segment = segments[chunk];
+  ChunkTest test{};
+  test.mode = kTestNone;
+  if (segment.row_count > 0) {
+    if (segment.encoding != HYB_ENC_DICTIONARY) {
+      test.mode = kTestInList;
+      test.negate = negate;
+    } else {
+      uint32_t* chunk_bits = bits ? bits + word_offsets[chunk] : nullptr;
+      if (list.compare == kInInt32) {
+        in_dictionary_test<AsInt32>(segment, list, negate, chunk_bits, test);
+      } else if (list.compare == kInInt64) {
+        in_dictionary_test<AsInt64>(segment, list, negate, chunk_bits, test);
+      } else if (list.compare == kInFloat) {
+        in_dictionary_test<AsFloat>(segment, list, negate, chunk_bits, test);
+      } else {
+        in_dictionary_test<AsDouble>(segment, list, negate, chunk_bits, test);
+      }
+    }
+  }
+  tests[chunk] = test;
+}
+
+// The device copy of a numeric list's intervals in its compare type; a list that matches no value of the column becomes
+// one empty interval (lo > hi), so a search always has an interval to land on.
+template <typename T, typename Member>
+static int upload_intervals(hyb_context* context, const std::vector<hyb_value>& bounds, Member hyb_value::*member_of,
+                            DeviceScratch& scratch, InList& list, uint64_t* out_bytes) {
+  std::vector<T> typed;
+  for (const hyb_value& bound : bounds) typed.push_back(static_cast<T>(bound.*member_of));
+  if (typed.empty()) typed = {T(1), T(0)};
+  T* device = nullptr;
+  HYB_TRY(scratch.alloc_array(typed.size(), &device));
+  // pageable source: the copy is staged before cudaMemcpyAsync returns
+  HYB_CUDA(cudaMemcpyAsync(device, typed.data(), sizeof(T) * typed.size(), cudaMemcpyHostToDevice, context->stream));
+  list.bounds = device;
+  list.interval_count = static_cast<uint32_t>(typed.size() / 2);
+  *out_bytes = sizeof(T) * typed.size();
+  return HYB_OK;
 }
 
 }  // namespace hyb
@@ -1506,6 +1693,169 @@ int hyb_table_scan_columns(hyb_context* context, hyb_table_t table_handle, const
     HYB_CUDA(cudaGetLastError());
   } else {
     HYB_TRY(launch_filtered<PairRows>(context, filter, left_segments, nullptr, extra, false, result.get(), &input_rows));
+    input_bytes += input_rows * sizeof(hyb_row_id);
+    launches = 3;
+  }
+  timing_end(context, launches, input_bytes, input_rows, 0);
+  timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
+
+  const auto handle = context->next_handle++;
+  context->pos_lists.emplace(handle, std::move(result));
+  *out_pos_list = handle;
+  return HYB_OK;
+}
+
+int hyb_table_scan_in(hyb_context* context, hyb_table_t table_handle, const hyb_in_predicate* predicate,
+                      hyb_pos_list_t input_filter, hyb_pos_list_t* out_pos_list) {
+  HYB_CHECK(context && predicate && out_pos_list, HYB_ERR_INVALID, "NULL argument");
+  *out_pos_list = 0;
+  DeviceGuard guard(context->device);
+  std::lock_guard<std::mutex> lock(context->mutex);
+  auto* table = find_table(context, table_handle);
+  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  PosList* filter = nullptr;
+  if (input_filter) {
+    filter = find_pos_list(context, input_filter);
+    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
+    HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
+  }
+  const int32_t condition = predicate->condition;
+  HYB_CHECK(condition == HYB_PRED_IN || condition == HYB_PRED_NOT_IN, HYB_ERR_INVALID,
+            "hyb_table_scan_in takes IN or NOT IN (condition " + std::to_string(condition) + ")");
+  HYB_CHECK(predicate->column_id < table->column_count, HYB_ERR_INVALID, "IN scan column out of range");
+  const int32_t data_type = table->column_types[predicate->column_id];
+  const bool strings = data_type == HYB_TYPE_STRING;
+  const bool negate = condition == HYB_PRED_NOT_IN;
+  HYB_CHECK(strings || !predicate->dictionary_matches, HYB_ERR_INVALID,
+            "dictionary_matches is for string columns; a numeric column takes its elements");
+
+  // Rules 1-3 of the header: which elements count, and whether the list reduces to "no row" or "every row".
+  std::vector<hyb_value> bounds;
+  bool compatible;
+  if (strings) {
+    compatible = predicate->dictionary_matches != nullptr;
+  } else {
+    HYB_TRY(normalize_in_list(data_type, predicate->elements, predicate->element_count, bounds));
+    compatible = predicate->element_count > 0 || predicate->has_null_element;
+  }
+  enum { kNoRow, kEveryRow, kList } form = kList;
+  if (!compatible) {
+    form = negate ? kEveryRow : kNoRow;  // `x IN ()` is false, `x NOT IN ()` is true, NULL rows included
+  } else if (!strings && negate && predicate->has_null_element) {
+    form = kNoRow;  // `x != NULL` is NULL: no row satisfies the conjunction
+  }
+  HYB_TRY(sync_table_descriptors(context, table));
+
+  timing_begin(context);
+  DeviceScratch scratch(context);
+  const uint32_t chunk_count = table->chunk_count();
+  const DevSegment* column_segments = table->d_segments + size_t{predicate->column_id} * chunk_count;
+  ChunkTest* tests = nullptr;
+  HYB_TRY(scratch.alloc_array(chunk_count, &tests));
+  InList list{};
+  list.interval_count = 1;
+  uint64_t list_bytes = 0;
+  if (form != kList) {
+    std::vector<ChunkTest> host(chunk_count);
+    for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+      host[chunk] = ChunkTest{};
+      const bool rows = table->segments[size_t{chunk} * table->column_count + predicate->column_id].row_count > 0;
+      host[chunk].mode = form == kEveryRow && rows ? kTestAll : kTestNone;
+    }
+    if (chunk_count) {
+      HYB_CUDA(cudaMemcpyAsync(tests, host.data(), sizeof(ChunkTest) * chunk_count, cudaMemcpyHostToDevice, context->stream));
+    }
+  } else if (strings) {
+    void* bitmap_scratch = nullptr;
+    uint64_t words = 0;
+    const int status = prepare_bitmap_tests(context, table, predicate->column_id, predicate->dictionary_matches, tests,
+                                            &bitmap_scratch, &words);
+    scratch.adopt(bitmap_scratch);
+    HYB_TRY(status);
+    list_bytes = sizeof(uint32_t) * words;
+  } else {
+    if (data_type == HYB_TYPE_INT32) {
+      list.compare = kInInt32;
+      HYB_TRY(upload_intervals<int32_t>(context, bounds, &hyb_value::i32, scratch, list, &list_bytes));
+    } else if (data_type == HYB_TYPE_INT64) {
+      list.compare = kInInt64;
+      HYB_TRY(upload_intervals<long long>(context, bounds, &hyb_value::i64, scratch, list, &list_bytes));
+    } else if (data_type == HYB_TYPE_FLOAT32) {
+      list.compare = kInFloat;
+      HYB_TRY(upload_intervals<float>(context, bounds, &hyb_value::f32, scratch, list, &list_bytes));
+    } else {
+      list.compare = kInDouble;
+      HYB_TRY(upload_intervals<double>(context, bounds, &hyb_value::f64, scratch, list, &list_bytes));
+    }
+    // bitmap words of the dictionary chunks, in case their value-IDs do not form one run
+    std::vector<unsigned long long> word_offsets(std::max<uint32_t>(chunk_count, 1), 0);
+    unsigned long long words = 0;
+    for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+      const DevSegment& segment = table->segments[size_t{chunk} * table->column_count + predicate->column_id];
+      word_offsets[chunk] = words;
+      if (segment.encoding == HYB_ENC_DICTIONARY) words += (size_t{segment.dict_size} + 31) / 32;
+    }
+    uint32_t* bits = nullptr;
+    unsigned long long* d_word_offsets = nullptr;
+    if (words > 0) {
+      HYB_TRY(scratch.alloc_array(words, &bits));
+      HYB_TRY(scratch.alloc_array(word_offsets.size(), &d_word_offsets));
+      HYB_CUDA(cudaMemcpyAsync(d_word_offsets, word_offsets.data(), sizeof(unsigned long long) * word_offsets.size(),
+                               cudaMemcpyHostToDevice, context->stream));
+    }
+    if (chunk_count) {
+      in_prepare_kernel<<<(chunk_count + 127) / 128, 128, 0, context->stream>>>(column_segments, chunk_count, list, negate,
+                                                                                d_word_offsets, bits, tests);
+      HYB_CUDA(cudaGetLastError());
+    }
+  }
+
+  auto result = std::make_unique<PosList>();
+  result->table = table_handle;
+  result->chunk_count = chunk_count;
+  result->stream = context->stream;
+  result->owner = context;
+  uint32_t launches = 1;
+  uint64_t input_rows = 0, input_bytes = list_bytes;
+  void* chunk_end = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
+  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
+
+  if (!filter) {
+    // IN lists only have the two-pass pipeline: scan_two_pass = 0 and scan_bulk select one-column kernels only.
+    if (context->options.trace && (!context->options.scan_two_pass || context->options.scan_bulk)) {
+      std::fprintf(stderr, "[hyb] hyb_table_scan_in: two-pass pipeline (IN lists have no single-pass or bulk kernel)\n");
+    }
+    const uint2* tile_map = nullptr;
+    uint32_t tile_count = 0;
+    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
+    input_rows = table->row_count();
+    input_bytes += column_bytes_per_launch(table, predicate->column_id);
+    result->capacity = table->row_count();
+    void* out = nullptr;
+    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
+    result->d_row_ids = static_cast<hyb_row_id*>(out);
+    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
+    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
+    timing_kernel_begin(context);
+    if (tile_count > 0) {
+      ScanParams params{};
+      params.segments = column_segments;
+      params.tests = tests;
+      params.tile_map = tile_map;
+      params.chunk_count = chunk_count;
+      params.tile_count = tile_count;
+      params.out = result->d_row_ids;
+      params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
+      HYB_TRY(launch_two_pass<InRows>(context, params, list));
+      launches = 4;
+    }
+    timing_kernel_end(context);
+    HYB_CUDA(cudaGetLastError());
+  } else {
+    // a NULL_ROW_ID reads as NULL: it matches only where NULL rows do, i.e. NOT IN over a list without a compatible element
+    HYB_TRY(launch_filtered<InRows>(context, filter, column_segments, tests, list, form == kEveryRow, result.get(),
+                                    &input_rows));
     input_bytes += input_rows * sizeof(hyb_row_id);
     launches = 3;
   }

@@ -62,6 +62,77 @@ def build_column_scan_predicate(table: Table, comparison: ColumnComparison, righ
     return struct, keepalive
 
 
+@dataclass
+class InList:
+    """column [NOT] IN (elements) — the literal list of an InExpression (condition PRED_IN or PRED_NOT_IN). Elements are
+    typed the way Hyrise types SQL literals (literal_type): int -> int32 if it fits, else int64; float -> double;
+    np.float32 -> float; str / bytes -> string; None -> NULL."""
+
+    column_id: int
+    condition: int
+    elements: Sequence = ()
+
+
+def literal_type(element) -> tuple[int | None, object]:
+    """(hyb data type, value) of one IN list element; (None, None) for NULL. Strings come back as bytes (str: UTF-8)."""
+    if element is None:
+        return None, None
+    if isinstance(element, (bool, np.bool_)):
+        raise TypeError("a boolean is not a SQL literal of Hyrise")
+    if isinstance(element, (str, bytes, np.bytes_)):
+        return capi.TYPE_STRING, element.encode() if isinstance(element, str) else bytes(element)
+    if isinstance(element, np.float32):
+        return capi.TYPE_FLOAT32, float(element)
+    if isinstance(element, np.int32):
+        return capi.TYPE_INT32, int(element)
+    if isinstance(element, np.int64):
+        return capi.TYPE_INT64, int(element)
+    if isinstance(element, (int, np.integer)):
+        value = int(element)
+        if -2**31 <= value < 2**31:
+            return capi.TYPE_INT32, value
+        if -2**63 <= value < 2**63:
+            return capi.TYPE_INT64, value
+        raise OverflowError(f"{value} exceeds int64")
+    if isinstance(element, (float, np.floating)):
+        return capi.TYPE_FLOAT64, float(element)
+    raise TypeError(f"unsupported IN list element {element!r}")
+
+
+def build_in_predicate(table: Table, in_list: InList, dictionary_matches: np.ndarray | None = None,
+                       ) -> tuple[capi.InPredicate, object]:
+    """The C struct plus an object that must stay alive while it is in use. A string column gets the dictionary bitmaps
+    of its string elements (Table.string_in_bitmaps) unless `dictionary_matches` is given, and none when the list has no
+    string element; a numeric column gets its numeric elements and whether the list holds a NULL (its string elements
+    are dropped, as the reference drops them)."""
+    struct = capi.InPredicate()
+    struct.column_id = in_list.column_id
+    struct.condition = in_list.condition
+    typed = [literal_type(element) for element in in_list.elements]
+    definitions = table.column_definitions
+    strings = in_list.column_id < len(definitions) and definitions[in_list.column_id].data_type == capi.TYPE_STRING
+    if strings:
+        string_elements = [value for data_type, value in typed if data_type == capi.TYPE_STRING]
+        if dictionary_matches is None and string_elements:
+            dictionary_matches = table.string_in_bitmaps(in_list.column_id, in_list.condition, string_elements)
+        keepalive = None
+        if dictionary_matches is not None:
+            keepalive = np.zeros(max(len(dictionary_matches), 1), dtype=np.uint32)  # never NULL, even without entries
+            keepalive[: len(dictionary_matches)] = dictionary_matches
+            struct.dictionary_matches = keepalive.ctypes.data
+        return struct, keepalive
+    numeric = [(data_type, value) for data_type, value in typed if data_type not in (None, capi.TYPE_STRING)]
+    elements = capi.literal_array(numeric)
+    struct.element_count = len(numeric)
+    struct.has_null_element = int(any(data_type is None for data_type, _ in typed))
+    struct.elements = C.cast(elements, C.POINTER(capi.Literal))
+    if dictionary_matches is not None:  # bitmaps on a numeric column: the library rejects them
+        words = np.ascontiguousarray(dictionary_matches, dtype=np.uint32)
+        struct.dictionary_matches = words.ctypes.data
+        return struct, (elements, words)
+    return struct, elements
+
+
 def _set_value(target: capi.Value, data_type: int, value) -> None:
     if value is None:
         return
@@ -363,6 +434,17 @@ class DeviceContext:
         handle = C.c_uint64()
         check(self.lib.hyb_table_scan_columns(self.ptr, table.handle, C.byref(struct),
                                               input_filter.handle if input_filter else 0, C.byref(handle)))
+        del keepalive
+        return DevicePosList(self, handle.value)
+
+    def table_scan_in(self, table: DeviceTable, in_list: InList, input_filter: DevicePosList | None = None,
+                      dictionary_matches: np.ndarray | None = None) -> DevicePosList:
+        """hyb_table_scan_in: `column [NOT] IN (elements)` per row. String columns build the dictionary bitmaps of the
+        host table unless `dictionary_matches` is given (e.g. NativeBinaryTable.in_bitmaps)."""
+        struct, keepalive = build_in_predicate(table.host_table, in_list, dictionary_matches)
+        handle = C.c_uint64()
+        check(self.lib.hyb_table_scan_in(self.ptr, table.handle, C.byref(struct),
+                                         input_filter.handle if input_filter else 0, C.byref(handle)))
         del keepalive
         return DevicePosList(self, handle.value)
 

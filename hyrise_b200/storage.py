@@ -372,6 +372,14 @@ class Table:
                  for chunk in self.chunks]
         return np.concatenate(words) if words else np.zeros(0, dtype=np.uint32)
 
+    def string_in_bitmaps(self, column_id: int, condition: int, elements) -> np.ndarray:
+        """dictionary_matches of `<string column> [NOT] IN (elements)`: per chunk, hyb_in_dictionary_matches of the
+        dictionary against the string elements (bytes), ceil(dictionary size / 32) uint32 words per chunk in chunk order;
+        NOT IN is inverted."""
+        words = [capi.in_dictionary_matches(condition, elements, chunk.segments[column_id].string_dictionary)
+                 for chunk in self.chunks]
+        return np.concatenate(words) if words else np.zeros(0, dtype=np.uint32)
+
     def string_column_translation(self, left_column_id: int, right_column_id: int) -> np.ndarray:
         """right_in_left of `left <condition> right` on two string columns: per chunk, hyb_dictionary_translate of the
         right dictionary into the left one's value-ID space, one uint32 word per right dictionary entry, in chunk order."""

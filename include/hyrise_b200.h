@@ -23,7 +23,7 @@
  *   - plain C: pointers + sizes, no C++/torch types; every function returns hyb_status (0 = OK);
  *     hyb_last_error() returns a thread-local message. No exception crosses this boundary.
  *   - every entry point is thread-safe and re-entrant; inputs are borrowed and immutable for the duration of the call.
- *   - HYB_ERR_UNSUPPORTED means "run the CPU operator" (e.g. IN scans, string join keys); anything else is a
+ *   - HYB_ERR_UNSUPPORTED means "run the CPU operator" (e.g. IN over a subquery, string join keys); anything else is a
  *     hard failure the shim turns into Fail(hyb_last_error()).
  *   - results stay device-resident behind handles (so the next operator can consume them without a PCIe round trip)
  *     and are copied out on request into caller-owned host memory (pinned via hyb_host_alloc for full PCIe speed).
@@ -102,8 +102,8 @@ typedef enum hyb_predicate_condition {
   HYB_PRED_BETWEEN_LOWER_EXCLUSIVE = 7,
   HYB_PRED_BETWEEN_UPPER_EXCLUSIVE = 8,
   HYB_PRED_BETWEEN_EXCLUSIVE = 9,
-  HYB_PRED_IN = 10,                   /* unsupported */
-  HYB_PRED_NOT_IN = 11,               /* unsupported */
+  HYB_PRED_IN = 10,                   /* hyb_table_scan_in; unsupported in hyb_scan_predicate */
+  HYB_PRED_NOT_IN = 11,               /* hyb_table_scan_in; unsupported in hyb_scan_predicate */
   HYB_PRED_LIKE = 12,                 /* STRING dictionary columns: value_id_bounds = match bitmaps */
   HYB_PRED_NOT_LIKE = 13,             /* STRING dictionary columns: value_id_bounds = match bitmaps */
   HYB_PRED_LIKE_INSENSITIVE = 14,     /* STRING dictionary columns: value_id_bounds = match bitmaps */
@@ -403,6 +403,71 @@ int hyb_table_scan_columns(hyb_context* context, hyb_table_t table, const hyb_co
 int hyb_dictionary_translate(const char* left_chars, const uint64_t* left_offsets, uint32_t left_count,
                              const char* right_chars, const uint64_t* right_offsets, uint32_t right_count,
                              uint32_t* out_words);
+
+/*
+ * <column> [NOT] IN (<literal>, ...): ExpressionEvaluator::_evaluate_in_expression (expression_evaluator.cpp:404-511) on a
+ * list of literals, the predicate the ExpressionEvaluatorTableScanImpl fallback scans. A row is selected iff the result is
+ * non-zero and not NULL:
+ *   1. Only type-compatible elements count: on a STRING column the string elements (NULL elements are dropped, their type
+ *      is Null); on a numeric column the numeric and the NULL elements (string elements are dropped).
+ *   2. No compatible element (the empty list included): IN selects no row, NOT IN selects every row, NULL rows and the
+ *      NULL_ROW_IDs of an outer join's PosList included (the result is an unnullable literal TRUE).
+ *   3. Otherwise a NULL value never matches; IN matches iff the value equals some non-NULL element; NOT IN iff it equals
+ *      no element and the compatible list holds no NULL (numeric `a NOT IN (1, NULL)` selects nothing).
+ *   4. Equality is std::equal_to in std::common_type_t<column type, element type>, as for hyb_table_scan_columns: int x int
+ *      in int64, int x float in float (the integer rounded to nearest), anything x double in double (an int64 rounded);
+ *      NaN equals nothing, -0.0 equals +0.0. So `float_col IN (0.05)` matches no row, `int64_col IN (2^53 as double)`
+ *      matches 2^53 and 2^53 + 1.
+ * The library applies rules 1-3. A STRING column ignores `elements` and `has_null_element` and takes per-chunk dictionary
+ * bitmaps in the layout of the LIKE conditions of hyb_scan_predicate (hyb_in_dictionary_matches, inverted for NOT IN);
+ * dictionary_matches == NULL means "the list has no string element". A numeric column takes its numeric elements (any
+ * numeric type, any order, duplicates allowed) and needs dictionary_matches == NULL; a caller leaves its string elements
+ * out (the struct cannot express them, and rule 1 drops them). HYB_ERR_INVALID: a condition other than HYB_PRED_IN /
+ * HYB_PRED_NOT_IN, a column id out of range, a non-numeric hyb_literal, or bitmaps on a numeric column. The output and
+ * `input_filter` behave exactly as for hyb_table_scan. HYB_PRED_IN / NOT_IN inside a hyb_scan_predicate (scans and fused
+ * aggregate predicates) stay HYB_ERR_UNSUPPORTED: an aggregate consumes this call's PosList through its `filter`.
+ */
+typedef struct hyb_in_predicate {
+  uint32_t column_id;
+  int32_t condition;                  /* HYB_PRED_IN | HYB_PRED_NOT_IN */
+  uint32_t element_count;             /* numeric literals in `elements` */
+  uint32_t has_null_element;          /* the list holds a NULL literal */
+  const hyb_literal* elements;        /* numeric elements: any numeric type, any order, duplicates allowed */
+  const uint32_t* dictionary_matches; /* STRING columns: per-chunk bitmaps; NULL = the list has no string element */
+} hyb_in_predicate;
+int hyb_table_scan_in(hyb_context* context, hyb_table_t table, const hyb_in_predicate* predicate,
+                      hyb_pos_list_t input_filter, hyb_pos_list_t* out_pos_list);
+
+/*
+ * Membership of every entry of one string dictionary in a list of strings (host only, no GPU): bytewise equality, as
+ * std::string's operator==. Elements and dictionary use the layout of hyb_dictionary_translate (chars may be NULL when
+ * every entry is empty); the elements may come in any order and repeat. out_words receives ceil(dictionary_count / 32)
+ * words, bit (i & 31) of word (i >> 5) set iff entry i is in the list (HYB_PRED_IN) or is not (HYB_PRED_NOT_IN, inverted
+ * as the NOT LIKE variants are), padding bits cleared; out_match_count (optional) the number of set bits. The caller
+ * passes hyb_in_predicate.dictionary_matches = NULL instead when the list has no string element (rule 2 above).
+ */
+int hyb_in_dictionary_matches(int32_t condition, const char* element_chars, const uint64_t* element_offsets,
+                              uint32_t element_count, const char* dictionary_chars, const uint64_t* dictionary_offsets,
+                              uint32_t dictionary_count, uint32_t* out_words, uint32_t* out_match_count);
+
+/* hyb_in_predicate.dictionary_matches for a string column of a parsed binary table: hyb_in_dictionary_matches over every
+ * chunk's dictionary, concatenated in chunk order. out_words == NULL: only *inout_word_count is set, to the number of
+ * words needed; otherwise *inout_word_count must be at least that. */
+int hyb_binary_table_in_bitmaps(const hyb_binary_table* table, uint32_t column, int32_t condition, const char* element_chars,
+                                const uint64_t* element_offsets, uint32_t element_count, uint32_t* out_words,
+                                uint32_t* inout_word_count);
+
+/*
+ * The numeric list of an IN predicate as the values of `column_type` it matches under rule 4 (host only, no GPU): sorted,
+ * disjoint closed intervals [lo, hi] in the column's type, out_bounds[2 * i] = lo and out_bounds[2 * i + 1] = hi (the
+ * member of hyb_value that column_type names). NaN elements vanish, -0.0 and +0.0 form one interval (stored as +0.0), an
+ * element that no value of the column type equals (0.05 against a float column, 2^40 against int32) vanishes, and a double
+ * or float element against an integer column can cover several integers. Intervals that touch are merged. On entry
+ * *inout_interval_count is the capacity of out_bounds in intervals (count <= capacity suffices); on return it is the
+ * number of intervals. out_bounds == NULL: only the count is returned. HYB_ERR_INVALID: a non-numeric column or element.
+ */
+int hyb_in_list_normalize(int32_t column_type, const hyb_literal* elements, uint32_t count, hyb_value* out_bounds,
+                          uint32_t* inout_interval_count);
 
 /* Total matches and per-chunk boundaries: out_chunk_offsets has chunk_count + 1 entries; chunk c's RowIDs are
  * [out_chunk_offsets[c], out_chunk_offsets[c+1]) of the flat list. Either pointer may be NULL. */

@@ -49,6 +49,8 @@ enum class PredicateCondition : int32_t {  // types.hpp:160-179
   BetweenLowerExclusive = HYB_PRED_BETWEEN_LOWER_EXCLUSIVE,
   BetweenUpperExclusive = HYB_PRED_BETWEEN_UPPER_EXCLUSIVE,
   BetweenExclusive = HYB_PRED_BETWEEN_EXCLUSIVE,
+  In = HYB_PRED_IN,        // InList (hyb_table_scan_in) only
+  NotIn = HYB_PRED_NOT_IN,  // InList (hyb_table_scan_in) only
   IsNull = HYB_PRED_IS_NULL,
   IsNotNull = HYB_PRED_IS_NOT_NULL
 };
@@ -150,6 +152,26 @@ class BinaryTable {
     check(hyb_binary_table_like_bitmaps(_table, column, pattern.data(), pattern.size(), condition, nullptr, &words));
     std::vector<uint32_t> bitmaps(std::max<uint32_t>(words, 1));
     check(hyb_binary_table_like_bitmaps(_table, column, pattern.data(), pattern.size(), condition, bitmaps.data(), &words));
+    return bitmaps;
+  }
+  // hyb_in_predicate.dictionary_matches of `<string column> [NOT] IN (elements)`: every chunk's dictionary entries that
+  // the list holds (inverted for NotIn), by bytewise equality (hyb_in_dictionary_matches)
+  std::vector<uint32_t> in_value_id_bitmaps(uint32_t column, PredicateCondition condition,
+                                            const std::vector<std::string>& elements) const {
+    std::string chars;
+    std::vector<uint64_t> offsets{0};
+    for (const auto& element : elements) {
+      chars += element;
+      offsets.push_back(chars.size());
+    }
+    const auto count = static_cast<uint32_t>(elements.size());
+    const char* data = chars.empty() ? nullptr : chars.data();
+    uint32_t words = 0;
+    check(hyb_binary_table_in_bitmaps(_table, column, static_cast<int32_t>(condition), data, offsets.data(), count, nullptr,
+                                      &words));
+    std::vector<uint32_t> bitmaps(std::max<uint32_t>(words, 1));
+    check(hyb_binary_table_in_bitmaps(_table, column, static_cast<int32_t>(condition), data, offsets.data(), count,
+                                      bitmaps.data(), &words));
     return bitmaps;
   }
   // hyb_column_scan_predicate.right_in_left of `left <condition> right` on two string columns: every chunk's right
@@ -398,11 +420,44 @@ struct ColumnComparison {
   }
 };
 
+// column [NOT] IN (<literal>, ...) (ExpressionEvaluator::_evaluate_in_expression on a literal list): condition is In or
+// NotIn. A numeric column takes the list's numeric literals (any numeric type, compared in the common type) and whether it
+// holds a NULL; its string literals are dropped. A string column takes the dictionary bitmaps of the list's string
+// literals (BinaryTable::in_value_id_bitmaps, hyb_in_dictionary_matches) and has_string_element; without a string element
+// the bitmaps stay empty. The library applies the reference's rules for NULL and for lists without a compatible element.
+struct InList {
+  ColumnID column_id;
+  PredicateCondition condition;
+  std::vector<AllTypeVariant> numeric_elements;
+  bool has_null_element = false;
+  bool has_string_element = false;
+  std::vector<uint32_t> dictionary_matches;
+
+  hyb_in_predicate to_abi(std::vector<hyb_literal>& literals) const {
+    literals.clear();
+    for (const auto& element : numeric_elements) {
+      literals.push_back(hyb_literal{static_cast<int32_t>(data_type_from_all_type_variant(element)), detail::to_value(element)});
+    }
+    if (has_string_element && dictionary_matches.empty()) {
+      throw std::invalid_argument("a string IN list needs its dictionary bitmaps (BinaryTable::in_value_id_bitmaps)");
+    }
+    hyb_in_predicate predicate{};
+    predicate.column_id = column_id;
+    predicate.condition = static_cast<int32_t>(condition);
+    predicate.element_count = static_cast<uint32_t>(literals.size());
+    predicate.has_null_element = has_null_element;
+    predicate.elements = literals.empty() ? nullptr : literals.data();
+    predicate.dictionary_matches = has_string_element ? dictionary_matches.data() : nullptr;
+    return predicate;
+  }
+};
+
 class TableScan : public Operator<PosListSet> {
  public:
   TableScan(OperatorInput input, ScanPredicate predicate) : _input(std::move(input)), _predicate(std::move(predicate)) {}
   TableScan(OperatorInput input, ColumnComparison comparison)
       : _input(std::move(input)), _comparison(std::move(comparison)) {}
+  TableScan(OperatorInput input, InList in_list) : _input(std::move(input)), _in_list(std::move(in_list)) {}
 
  protected:
   std::shared_ptr<const PosListSet> _on_execute() override {
@@ -411,6 +466,10 @@ class TableScan : public Operator<PosListSet> {
     if (_comparison) {
       const auto abi = _comparison->to_abi();
       check(hyb_table_scan_columns(context, _input.table->handle(), &abi, _input.filter_handle(), &handle));
+    } else if (_in_list) {
+      std::vector<hyb_literal> literals;
+      const auto abi = _in_list->to_abi(literals);
+      check(hyb_table_scan_in(context, _input.table->handle(), &abi, _input.filter_handle(), &handle));
     } else {
       const auto abi = _predicate->to_abi();
       check(hyb_table_scan(context, _input.table->handle(), &abi, _input.filter_handle(), &handle));
@@ -423,6 +482,7 @@ class TableScan : public Operator<PosListSet> {
   OperatorInput _input;
   std::optional<ScanPredicate> _predicate;
   std::optional<ColumnComparison> _comparison;
+  std::optional<InList> _in_list;
 };
 
 // operator_join_predicate.hpp:16-44 — JoinHash supports exactly one equality predicate on the device.

@@ -5,7 +5,10 @@
 #include "device_column_pool.hpp"
 #include "expression/evaluation/like_matcher.hpp"
 #include "expression/expression_utils.hpp"
+#include "expression/in_expression.hpp"
+#include "expression/list_expression.hpp"
 #include "expression/pqp_column_expression.hpp"
+#include "expression/value_expression.hpp"
 #include "expression/window_function_expression.hpp"
 #include "hyrise_b200.h"
 #include "operators/join_helper/join_output_writing.hpp"
@@ -107,23 +110,28 @@ bool like_dictionary_bitmaps(const Table& stored, ColumnID column_id, PredicateC
 // hyb_column_scan_predicate.right_in_left: per chunk, every right dictionary entry as 2 * lower_bound in the left dictionary
 // + (found ? 1 : 0), one merge of the two sorted dictionaries; one word per right entry, chunk after chunk. Only
 // DictionarySegment<pmr_string> / FixedStringDictionarySegment dictionaries (false: the CPU operator runs).
+// The sorted dictionary of a string segment (DictionarySegment<pmr_string> or FixedStringDictionarySegment), or nullopt.
+std::optional<std::vector<pmr_string>> string_dictionary(const Table& stored, const ChunkID chunk_id, const ColumnID column_id) {
+  const auto segment = stored.get_chunk(chunk_id)->get_segment(column_id);
+  if (const auto dictionary_segment = std::dynamic_pointer_cast<const DictionarySegment<pmr_string>>(segment)) {
+    const auto& dictionary = *dictionary_segment->dictionary();
+    return std::vector<pmr_string>(dictionary.begin(), dictionary.end());
+  }
+  if (const auto fixed_segment = std::dynamic_pointer_cast<const FixedStringDictionarySegment<pmr_string>>(segment)) {
+    const auto& dictionary = *fixed_segment->fixed_string_dictionary();
+    auto entries = std::vector<pmr_string>{};
+    entries.reserve(dictionary.size());
+    for (auto entry = size_t{0}; entry < dictionary.size(); ++entry) {
+      entries.emplace_back(dictionary.get_string_at(entry));
+    }
+    return entries;
+  }
+  return std::nullopt;
+}
+
 bool column_translation(const Table& stored, ColumnID left_column_id, ColumnID right_column_id, std::vector<uint32_t>& words) {
-  const auto dictionary_of = [&](const ChunkID chunk_id, const ColumnID column_id) -> std::optional<std::vector<pmr_string>> {
-    const auto segment = stored.get_chunk(chunk_id)->get_segment(column_id);
-    if (const auto dictionary_segment = std::dynamic_pointer_cast<const DictionarySegment<pmr_string>>(segment)) {
-      const auto& dictionary = *dictionary_segment->dictionary();
-      return std::vector<pmr_string>(dictionary.begin(), dictionary.end());
-    }
-    if (const auto fixed_segment = std::dynamic_pointer_cast<const FixedStringDictionarySegment<pmr_string>>(segment)) {
-      const auto& dictionary = *fixed_segment->fixed_string_dictionary();
-      auto entries = std::vector<pmr_string>{};
-      entries.reserve(dictionary.size());
-      for (auto entry = size_t{0}; entry < dictionary.size(); ++entry) {
-        entries.emplace_back(dictionary.get_string_at(entry));
-      }
-      return entries;
-    }
-    return std::nullopt;
+  const auto dictionary_of = [&](const ChunkID chunk_id, const ColumnID column_id) {
+    return string_dictionary(stored, chunk_id, column_id);
   };
   for (auto chunk_id = ChunkID{0}; chunk_id < stored.chunk_count(); ++chunk_id) {
     const auto left = dictionary_of(chunk_id, left_column_id);
@@ -268,6 +276,97 @@ std::shared_ptr<const Table> try_gpu_column_scan(const std::shared_ptr<const Tab
   const auto status = hyb_table_scan_columns(pool->context(), entry->handle, &predicate, 0, &result);
   if (status == HYB_ERR_UNSUPPORTED) {
     return nullptr;  // LIKE between two columns: the reference operator reports it itself
+  }
+  Assert(status == HYB_OK, hyb_last_error());
+  return wrap_pos_lists(pool->context(), in_table, result);
+}
+
+std::shared_ptr<const Table> try_gpu_in_scan(const std::shared_ptr<const Table>& in_table, const InExpression& in_expression) {
+  auto* pool = gpu_column_pool();
+  if (!pool || in_table->type() != TableType::Data) {
+    return nullptr;  // reference-table inputs: as in try_gpu_table_scan
+  }
+  const auto* entry = pool->find(in_table);
+  const auto column = std::dynamic_pointer_cast<const PQPColumnExpression>(in_expression.operand());
+  const auto list = std::dynamic_pointer_cast<const ListExpression>(in_expression.set());
+  if (!entry || !column || !list) {
+    return nullptr;  // IN over a subquery or an expression: ExpressionEvaluator
+  }
+  auto literals = std::vector<hyb_literal>{};
+  auto strings = std::vector<pmr_string>{};
+  auto has_null_element = false;
+  for (const auto& element : list->elements()) {
+    const auto value_expression = std::dynamic_pointer_cast<const ValueExpression>(element);
+    if (!value_expression) {
+      return nullptr;  // a non-literal element (`13 * 13`, a column, a parameter) stays on the CPU
+    }
+    const auto& value = value_expression->value;
+    if (variant_is_null(value)) {
+      has_null_element = true;
+    } else if (value.type() == typeid(pmr_string)) {
+      strings.emplace_back(boost::get<pmr_string>(value));
+    } else {
+      auto literal = hyb_literal{};
+      if (value.type() == typeid(int32_t)) {
+        literal.data_type = HYB_TYPE_INT32;
+        literal.value.i32 = boost::get<int32_t>(value);
+      } else if (value.type() == typeid(int64_t)) {
+        literal.data_type = HYB_TYPE_INT64;
+        literal.value.i64 = boost::get<int64_t>(value);
+      } else if (value.type() == typeid(float)) {
+        literal.data_type = HYB_TYPE_FLOAT32;
+        literal.value.f32 = boost::get<float>(value);
+      } else {
+        literal.data_type = HYB_TYPE_FLOAT64;
+        literal.value.f64 = boost::get<double>(value);
+      }
+      literals.push_back(literal);
+    }
+  }
+  auto predicate = hyb_in_predicate{};
+  predicate.column_id = column->column_id;
+  predicate.condition = in_expression.is_negated() ? HYB_PRED_NOT_IN : HYB_PRED_IN;
+  auto words = std::vector<uint32_t>{};
+  if (in_table->column_data_type(column->column_id) == DataType::String) {
+    // the library drops numeric and NULL elements of a string column itself; only the string elements become bitmaps
+    if (!strings.empty()) {
+      auto element_chars = std::string{};
+      auto element_offsets = std::vector<uint64_t>{0};
+      for (const auto& string : strings) {
+        element_chars.append(string.data(), string.size());
+        element_offsets.push_back(element_chars.size());
+      }
+      for (auto chunk_id = ChunkID{0}; chunk_id < in_table->chunk_count(); ++chunk_id) {
+        const auto dictionary = string_dictionary(*in_table, chunk_id, column->column_id);
+        if (!dictionary) {
+          return nullptr;
+        }
+        auto chars = std::string{};
+        auto offsets = std::vector<uint64_t>{0};
+        for (const auto& value : *dictionary) {
+          chars.append(value.data(), value.size());
+          offsets.push_back(chars.size());
+        }
+        const auto first = words.size();
+        words.resize(first + (dictionary->size() + 31) / 32);
+        Assert(hyb_in_dictionary_matches(predicate.condition, element_chars.data(), element_offsets.data(),
+                                         static_cast<uint32_t>(strings.size()), chars.data(), offsets.data(),
+                                         static_cast<uint32_t>(dictionary->size()), words.data() + first, nullptr) == HYB_OK,
+               hyb_last_error());
+      }
+      words.push_back(0);  // never a NULL pointer, even when no chunk has a dictionary entry
+      predicate.dictionary_matches = words.data();
+    }
+  } else {
+    // string elements of a numeric column are dropped, as rewrite_in_list_expression drops them
+    predicate.element_count = static_cast<uint32_t>(literals.size());
+    predicate.has_null_element = has_null_element;
+    predicate.elements = literals.data();
+  }
+  auto result = hyb_pos_list_t{};
+  const auto status = hyb_table_scan_in(pool->context(), entry->handle, &predicate, 0, &result);
+  if (status == HYB_ERR_UNSUPPORTED) {
+    return nullptr;
   }
   Assert(status == HYB_OK, hyb_last_error());
   return wrap_pos_lists(pool->context(), in_table, result);

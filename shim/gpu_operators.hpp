@@ -11,6 +11,7 @@
 namespace hyrise {
 
 class DeviceColumnPool;
+class InExpression;
 class WindowFunctionExpression;
 
 // Process-wide access for the operators (set by the plugin's start(), cleared by stop()). nullptr: no GPU path.
@@ -30,6 +31,11 @@ std::shared_ptr<const Table> try_gpu_table_scan(const std::shared_ptr<const Tabl
 // OperatorScanPredicate compares two columns of a stored table. String columns need dictionary segments.
 std::shared_ptr<const Table> try_gpu_column_scan(const std::shared_ptr<const Table>& in_table, ColumnID left_column_id,
                                                  PredicateCondition condition, ColumnID right_column_id);
+
+// TableScan::_on_execute when create_impl would fall back to an ExpressionEvaluatorTableScanImpl for
+// `<column> [NOT] IN (<literal>, ...)` (expression_evaluator.cpp:404-511): the operand is a column of a stored table and every
+// list element a ValueExpression. String columns need dictionary segments. Subqueries and non-literal elements: nullptr.
+std::shared_ptr<const Table> try_gpu_in_scan(const std::shared_ptr<const Table>& in_table, const InExpression& in_expression);
 
 // JoinHash::_on_execute (join_hash.cpp:116-225), after the build/probe side selection and the radix-bit calculation.
 std::shared_ptr<const Table> try_gpu_join_hash(const std::shared_ptr<const Table>& build_table,
