@@ -70,6 +70,12 @@ build/aggregate_distinct_check: tests/cpp/aggregate_distinct_check.cpp include/h
 	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/aggregate_distinct_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
 		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
 
+# String MIN / MAX / COUNT and ANY through the mirror on the GPU, over a reference binary fixture.
+build/string_aggregate_check: tests/cpp/string_aggregate_check.cpp include/hyrise_b200.hpp include/hyrise_b200.h $(LIB)
+	@mkdir -p build
+	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/string_aggregate_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
+		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
+
 # CPU restatement of the ExpressionEvaluator's IN over a literal list (test infrastructure, tests/in_scan_oracle.py).
 # No -ffast-math: NaN and signed zeros must compare as std::equal_to does.
 $(IN_SCAN_ORACLE): tests/cpp/in_scan_oracle.cpp include/hyrise_b200.h

@@ -415,6 +415,15 @@ class NativeBinaryTable:
                                                                 C.byref(count)))
         return words[: count.value]
 
+    def string_order_ranks(self, column: int) -> np.ndarray:
+        """hyb_binary_table_string_order_ranks: the order ranks of a string column (hyb_table_set_string_order's words)."""
+        count = C.c_uint32()
+        capi.check(self.lib.hyb_binary_table_string_order_ranks(self.ptr, column, None, C.byref(count)))
+        ranks = np.zeros(max(count.value, 1), dtype=np.uint32)
+        capi.check(self.lib.hyb_binary_table_string_order_ranks(self.ptr, column, ranks.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                                                C.byref(count)))
+        return ranks[: count.value]
+
     def host_blocks(self) -> list:
         count = C.c_uint32()
         capi.check(self.lib.hyb_binary_table_blocks(self.ptr, None, C.byref(count)))

@@ -208,6 +208,10 @@ SYMBOLS = {
     "hyb_like_dictionary_matches": [C.c_char_p, _U64, _I32, C.c_void_p, C.POINTER(_U64), _U32, C.POINTER(_U32),
                                     C.POINTER(_U32)],
     "hyb_dictionary_translate": [C.c_void_p, C.POINTER(_U64), _U32, C.c_void_p, C.POINTER(_U64), _U32, C.POINTER(_U32)],
+    "hyb_dictionary_order_ranks": [_U32, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(_U64)), C.POINTER(_U32), C.POINTER(_U32),
+                                   C.POINTER(_U32)],
+    "hyb_binary_table_string_order_ranks": [C.c_void_p, _U32, C.POINTER(_U32), C.POINTER(_U32)],
+    "hyb_table_set_string_order": [_CTX, _U64, _U32, C.POINTER(_U32), _U64],
     "hyb_table_scan": [_CTX, _U64, C.POINTER(ScanPredicate), _U64, C.POINTER(_U64)],
     "hyb_table_scan_columns": [_CTX, _U64, C.POINTER(ColumnScanPredicate), _U64, C.POINTER(_U64)],
     "hyb_table_scan_in": [_CTX, _U64, C.POINTER(InPredicate), _U64, C.POINTER(_U64)],
@@ -299,6 +303,26 @@ def dictionary_translate(left_entries, right_entries) -> "np.ndarray":
                                                   right_offsets.ctypes.data_as(C.POINTER(C.c_uint64)), count,
                                                   words.ctypes.data_as(C.POINTER(C.c_uint32))))
     return words[:count]
+
+
+def dictionary_order_ranks(dictionaries) -> tuple["np.ndarray", int]:
+    """hyb_dictionary_order_ranks: (ranks, distinct count) for sorted unique string dictionaries (sequences of bytes):
+    every entry's dense rank among the distinct strings of all of them, dictionary after dictionary. Host only."""
+    import numpy as np
+
+    arguments = [_string_dictionary_arguments(dictionary) for dictionary in dictionaries]
+    count = len(arguments)
+    chars = (C.c_void_p * max(count, 1))(*[C.cast(C.c_char_p(chars), C.c_void_p) if chars else None
+                                           for chars, _ in arguments])
+    offsets = (C.POINTER(C.c_uint64) * max(count, 1))(*[offsets.ctypes.data_as(C.POINTER(C.c_uint64))
+                                                         for _, offsets in arguments])
+    counts = (C.c_uint32 * max(count, 1))(*[len(offsets) - 1 for _, offsets in arguments])
+    total = sum(len(offsets) - 1 for _, offsets in arguments)
+    ranks = np.zeros(max(total, 1), dtype=np.uint32)
+    distinct = C.c_uint32()
+    check(load_library().hyb_dictionary_order_ranks(count, chars, offsets, counts, ranks.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                                    C.byref(distinct)))
+    return ranks[:total], distinct.value
 
 
 def in_dictionary_matches(condition: int, elements, entries) -> "np.ndarray":

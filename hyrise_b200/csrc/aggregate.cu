@@ -662,6 +662,40 @@ __global__ void aggregate_compact_kernel(const GroupTable table, uint32_t aggreg
   }
 }
 
+// String MIN / MAX: the general kernel accumulated the ordered encoding of the extreme order rank (the column's
+// StringColumnView turns its dictionaries into rank words). Before the occupied slots are packed, each such accumulator
+// becomes the hyb_dictionary_position {chunk_id, value_id} of the first dictionary entry holding that rank.
+struct StringExtremes {
+  const unsigned long long* first_entry[HYB_MAX_AGGREGATES];  // per aggregate: chunk << 32 | value-ID by rank, or nullptr
+};
+
+__global__ void string_extreme_kernel(const GroupTable table, uint32_t aggregate_count,
+                                      const __grid_constant__ StringExtremes extremes) {
+  const uint32_t capacity = table.capacity_mask + 1;
+  for (uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x; slot < capacity; slot += gridDim.x * blockDim.x) {
+    if (table.hashes[slot] == 0) continue;
+    for (uint32_t a = 0; a < aggregate_count; ++a) {
+      if (!extremes.first_entry[a] || table.counts[static_cast<size_t>(a) * capacity + slot] == 0) continue;
+      unsigned long long* accumulator = table.accumulators + static_cast<size_t>(a) * capacity + slot;
+      const uint32_t rank = static_cast<uint32_t>(*accumulator ^ 0x8000000000000000ull);
+      const unsigned long long entry = extremes.first_entry[a][rank];
+      *accumulator = (entry >> 32) | (entry << 32);
+    }
+  }
+}
+
+// Once per hyb_table_set_string_order: the first {chunk, value-ID} (in chunk order) of every rank, as chunk << 32 |
+// value-ID so that atomicMin keeps the first. One CTA per chunk.
+__global__ void string_order_first_entry_kernel(const uint32_t* __restrict__ ranks, const uint64_t* __restrict__ chunk_begin,
+                                                uint32_t chunk_count, unsigned long long* __restrict__ first_entry) {
+  for (uint32_t chunk = blockIdx.x; chunk < chunk_count; chunk += gridDim.x) {
+    const uint64_t begin = chunk_begin[chunk], end = chunk_begin[chunk + 1];
+    for (uint64_t entry = begin + threadIdx.x; entry < end; entry += blockDim.x) {
+      atomicMin(first_entry + ranks[entry], (static_cast<unsigned long long>(chunk) << 32) | (entry - begin));
+    }
+  }
+}
+
 __global__ void gather_row_ids_kernel(const unsigned long long* __restrict__ positions, uint32_t count,
                                       const hyb_row_id* __restrict__ filter, hyb_row_id* __restrict__ out) {
   const uint32_t index = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1817,6 +1851,109 @@ static int exchange_partial_groups_partitioned(hyb_context* context, const Aggre
                                                const hyb_aggregate_query* query, const std::vector<int32_t>& input_types,
                                                std::vector<HostGroup>* groups, int* out_immediate);
 
+// The INT32 dictionary descriptors of a string column (Table::StringColumnView) with `words` as per-chunk dictionaries:
+// chunk c's dictionary starts at words + word_begin[c] (word_begin == nullptr: every chunk reads `words` itself).
+static int build_string_view_segments(hyb_context* context, Table* table, uint32_t column, Table::StringColumnView* view,
+                                      const uint64_t* word_begin) {
+  const uint32_t chunk_count = table->chunk_count();
+  std::vector<DevSegment> segments(chunk_count);
+  for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+    DevSegment segment = table->segments[size_t{chunk} * table->column_count + column];
+    HYB_CHECK(segment.encoding == HYB_ENC_DICTIONARY, HYB_ERR_UNSUPPORTED, "string aggregates need dictionary segments");
+    segment.data_type = HYB_TYPE_INT32;  // dict_codes stay: COUNT(DISTINCT) of the same column reads them
+    segment.values = view->d_words + (word_begin ? word_begin[chunk] : 0);
+    segments[chunk] = segment;
+  }
+  HYB_TRY(device_alloc(context, sizeof(DevSegment) * std::max<uint32_t>(chunk_count, 1), reinterpret_cast<void**>(&view->d_segments)));
+  if (chunk_count) {
+    HYB_CUDA(cudaMemcpyAsync(view->d_segments, segments.data(), sizeof(DevSegment) * chunk_count, cudaMemcpyHostToDevice,
+                             context->stream));
+  }
+  HYB_CUDA(cudaStreamSynchronize(context->stream));
+  return HYB_OK;
+}
+
+// The view a string MIN / MAX (`need_order`) or COUNT reads. COUNT without attached ranks gets zero words: it tests the
+// value-ID against the NULL value-ID only.
+static int string_column_view(hyb_context* context, Table* table, uint32_t column, bool need_order,
+                              Table::StringColumnView** out_view) {
+  auto it = table->string_views.find(column);
+  if (it == table->string_views.end()) {
+    HYB_CHECK(!need_order, HYB_ERR_UNSUPPORTED,
+              "MIN / MAX over string column " + std::to_string(column) + " needs hyb_table_set_string_order");
+    auto view = std::make_shared<Table::StringColumnView>();
+    view->owner = context;
+    uint32_t max_dictionary = 0;
+    for (uint32_t chunk = 0; chunk < table->chunk_count(); ++chunk) {
+      max_dictionary = std::max(max_dictionary, table->segments[size_t{chunk} * table->column_count + column].dict_size);
+    }
+    HYB_TRY(device_alloc(context, sizeof(uint32_t) * (size_t{max_dictionary} + 1), reinterpret_cast<void**>(&view->d_words)));
+    HYB_CUDA(cudaMemsetAsync(view->d_words, 0, sizeof(uint32_t) * (size_t{max_dictionary} + 1), context->stream));
+    HYB_TRY(build_string_view_segments(context, table, column, view.get(), nullptr));
+    it = table->string_views.emplace(column, std::move(view)).first;
+  }
+  HYB_CHECK(!need_order || it->second->ordered, HYB_ERR_UNSUPPORTED,
+            "MIN / MAX over string column " + std::to_string(column) + " needs hyb_table_set_string_order");
+  *out_view = it->second.get();
+  return HYB_OK;
+}
+
+extern "C" int hyb_table_set_string_order(hyb_context* context, hyb_table_t handle, uint32_t column, const uint32_t* ranks,
+                                          uint64_t count) {
+  HYB_CHECK(context, HYB_ERR_INVALID, "context is NULL");
+  DeviceGuard guard(context->device);
+  std::lock_guard<std::mutex> lock(context->mutex);
+  auto* table = find_table(context, handle);
+  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  HYB_CHECK(column < table->column_count && table->column_types[column] == HYB_TYPE_STRING, HYB_ERR_INVALID,
+            "not a string column");
+  const uint32_t chunk_count = table->chunk_count();
+  std::vector<uint64_t> word_begin(size_t{chunk_count} + 1, 0);
+  for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+    const DevSegment& segment = table->segments[size_t{chunk} * table->column_count + column];
+    HYB_CHECK(segment.encoding == HYB_ENC_DICTIONARY, HYB_ERR_INVALID, "not a string dictionary column");
+    word_begin[chunk + 1] = word_begin[chunk] + segment.dict_size;
+  }
+  HYB_CHECK(count == word_begin.back(), HYB_ERR_INVALID,
+            "expected " + std::to_string(word_begin.back()) + " rank words (one per dictionary entry), got " + std::to_string(count));
+  HYB_CHECK(ranks || count == 0, HYB_ERR_INVALID, "ranks is NULL");
+  uint32_t max_rank = 0;
+  for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+    for (uint64_t word = word_begin[chunk]; word < word_begin[chunk + 1]; ++word) {
+      // dense ranks stay below the word count; that also bounds the rank -> first entry table by it
+      HYB_CHECK(ranks[word] < (1u << 31) && ranks[word] < count, HYB_ERR_INVALID,
+                "rank words must be below 2^31 and below their count");
+      HYB_CHECK(word == word_begin[chunk] || ranks[word] > ranks[word - 1], HYB_ERR_INVALID,
+                "rank words must be strictly increasing within chunk " + std::to_string(chunk));
+      max_rank = std::max(max_rank, ranks[word]);
+    }
+  }
+  HYB_TRY(sync_table_descriptors(context, table));  // before the view: a pending descriptor sync drops views
+  auto view = std::make_shared<Table::StringColumnView>();
+  view->owner = context;
+  view->ordered = true;
+  view->word_count = count;
+  const uint64_t distinct_bound = count ? uint64_t{max_rank} + 1 : 1;
+  HYB_TRY(device_alloc(context, sizeof(uint32_t) * std::max<uint64_t>(count, 1), reinterpret_cast<void**>(&view->d_words)));
+  HYB_TRY(device_alloc(context, sizeof(unsigned long long) * distinct_bound, reinterpret_cast<void**>(&view->d_first_entry)));
+  uint64_t* d_word_begin = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(uint64_t) * word_begin.size(), reinterpret_cast<void**>(&d_word_begin)));
+  DeviceScratch scratch(context);
+  scratch.adopt(d_word_begin);
+  if (count) HYB_CUDA(cudaMemcpyAsync(view->d_words, ranks, sizeof(uint32_t) * count, cudaMemcpyHostToDevice, context->stream));
+  HYB_CUDA(cudaMemcpyAsync(d_word_begin, word_begin.data(), sizeof(uint64_t) * word_begin.size(), cudaMemcpyHostToDevice,
+                           context->stream));
+  HYB_CUDA(cudaMemsetAsync(view->d_first_entry, 0xFF, sizeof(unsigned long long) * distinct_bound, context->stream));
+  if (chunk_count) {
+    string_order_first_entry_kernel<<<std::min<uint32_t>(chunk_count, context->sm_count * 8), 256, 0, context->stream>>>(
+        view->d_words, d_word_begin, chunk_count, view->d_first_entry);
+    HYB_CUDA(cudaGetLastError());
+  }
+  HYB_TRY(build_string_view_segments(context, table, column, view.get(), word_begin.data()));
+  table->string_views[column] = std::move(view);
+  return HYB_OK;
+}
+
 // Per (table, query shape): what the descriptor walk found. See Table::plan_memo.
 struct AggregatePlanMemo {
   uint64_t algorithmic_bytes = 0;
@@ -1864,8 +2001,44 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
   const uint32_t chunk_count = table->chunk_count();
   const uint32_t aggregate_count = query->aggregate_count;
 
+  // ---- ANY: a group-by column the shim writes from the representative RowIDs (write_groupby_output, :421-537) -------
+  // It adds no accumulator: the other aggregates run exactly as without it (an all-ANY query is the group-by-only call,
+  // the reference's DISTINCT path), and its column of the result only names its type.
+  std::vector<hyb_aggregate_def> kept;
+  std::vector<int32_t> any_types(aggregate_count, -1);
+  for (uint32_t a = 0; a < aggregate_count; ++a) {
+    const auto& def = query->aggregates[a];
+    if (def.function != HYB_AGG_ANY) {
+      kept.push_back(def);
+      continue;
+    }
+    HYB_CHECK(def.node_count == 1 && def.nodes[0].op == HYB_EXPR_COLUMN && def.nodes[0].column_id < table->column_count,
+              HYB_ERR_INVALID, "ANY takes a single column of the input table");
+    any_types[a] = table->column_types[def.nodes[0].column_id];
+  }
+  if (kept.size() < aggregate_count) {
+    hyb_aggregate_query reduced = *query;
+    reduced.aggregate_count = static_cast<uint32_t>(kept.size());
+    reduced.aggregates = kept.data();
+    HYB_TRY(aggregate_hash_locked(context, &reduced, out_result, exchange));
+    auto& result = *context->aggregate_results.at(*out_result);
+    std::vector<AggregateColumn> columns(aggregate_count);
+    for (uint32_t a = 0, next = 0; a < aggregate_count; ++a) {
+      if (any_types[a] >= 0) {
+        columns[a].value_type = any_types[a];
+        columns[a].is_any = true;
+      } else {
+        columns[a] = std::move(result.columns[next++]);
+      }
+    }
+    result.columns = std::move(columns);
+    return HYB_OK;
+  }
+
   // ---- validate + type the aggregates -----------------------------------------------------------------------------
   std::vector<int32_t> input_types(aggregate_count, HYB_TYPE_INT64), result_types(aggregate_count, HYB_TYPE_INT64);
+  // MIN / MAX / COUNT of a bare string column: the column's INT32 view (order ranks, or zeros for COUNT)
+  std::vector<Table::StringColumnView*> string_views(aggregate_count, nullptr);
   for (uint32_t a = 0; a < aggregate_count; ++a) {
     const auto& def = query->aggregates[a];
     HYB_CHECK(def.function >= HYB_AGG_MIN && def.function <= HYB_AGG_STDDEV_SAMP, HYB_ERR_UNSUPPORTED,
@@ -1892,6 +2065,14 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
       }
       input_types[a] = HYB_TYPE_STRING;
       result_types[a] = HYB_TYPE_INT64;
+      continue;
+    }
+    const bool bare_column = def.node_count == 1 && def.nodes[0].op == HYB_EXPR_COLUMN;
+    if (string_argument && bare_column &&
+        (def.function == HYB_AGG_MIN || def.function == HYB_AGG_MAX || def.function == HYB_AGG_COUNT)) {
+      HYB_TRY(string_column_view(context, table, def.nodes[0].column_id, def.function != HYB_AGG_COUNT, &string_views[a]));
+      input_types[a] = HYB_TYPE_STRING;
+      result_types[a] = def.function == HYB_AGG_COUNT ? HYB_TYPE_INT64 : HYB_TYPE_STRING;
       continue;
     }
     HYB_TRY(expression_type(table, def, &input_types[a]));
@@ -1974,8 +2155,27 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
         if (segment.nulls) memo->algorithmic_bytes += segment.row_count;
       }
     }
+    // string MIN / MAX read the column's rank words as its dictionaries
+    std::vector<const Table::StringColumnView*> ranked;
+    for (uint32_t a = 0; a < aggregate_count; ++a) {
+      if (string_views[a] && string_views[a]->ordered && result_types[a] == HYB_TYPE_STRING &&
+          std::find(ranked.begin(), ranked.end(), string_views[a]) == ranked.end()) {
+        ranked.push_back(string_views[a]);
+        memo->algorithmic_bytes += sizeof(uint32_t) * string_views[a]->word_count;
+      }
+    }
   }
   algorithmic_bytes = filter ? position_count * sizeof(hyb_row_id) : memo->algorithmic_bytes;
+  if (filter) {  // string MIN / MAX read their rank words as dictionaries on filtered inputs too
+    std::vector<const Table::StringColumnView*> ranked;
+    for (uint32_t a = 0; a < aggregate_count; ++a) {
+      if (string_views[a] && result_types[a] == HYB_TYPE_STRING &&
+          std::find(ranked.begin(), ranked.end(), string_views[a]) == ranked.end()) {
+        ranked.push_back(string_views[a]);
+        algorithmic_bytes += sizeof(uint32_t) * string_views[a]->word_count;
+      }
+    }
+  }
   bool kernel_timed = false;
 
   // ---- fast path --------------------------------------------------------------------------------------------------
@@ -2260,6 +2460,18 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
     for (size_t c = 0; c < plan_columns.size(); ++c) {
       host_plan.columns[c] = table->d_segments + size_t{plan_columns[c]} * chunk_count;
     }
+    // a string column that a MIN / MAX / COUNT reads is its INT32 view for every aggregate of the plan (the view keeps
+    // the dictionary codes a COUNT(DISTINCT) of the same column reads)
+    StringExtremes string_extremes{};
+    bool has_string_extremes = false;
+    for (uint32_t a = 0; a < aggregate_count; ++a) {
+      if (!string_views[a]) continue;
+      host_plan.columns[host_plan.aggregates[a].nodes[0].column] = string_views[a]->d_segments;
+      if (result_types[a] == HYB_TYPE_STRING) {
+        string_extremes.first_entry[a] = string_views[a]->d_first_entry;
+        has_string_extremes = true;
+      }
+    }
     void* device_plan = nullptr;
     HYB_TRY(device_alloc(context, sizeof(AggregatePlan), &device_plan));
     HYB_CUDA(cudaMemcpyAsync(device_plan, &host_plan, sizeof(AggregatePlan), cudaMemcpyHostToDevice, stream));
@@ -2390,6 +2602,13 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
         timing_kernel_end(context);
         launches += 2;
       }
+      if (has_string_extremes && table_control[0]) {
+        const uint32_t slot_grid =
+            static_cast<uint32_t>(std::min<uint64_t>((capacity + 255) / 256, static_cast<uint64_t>(context->sm_count) * 16));
+        string_extreme_kernel<<<slot_grid, 256, 0, stream>>>(group_table, aggregate_count, string_extremes);
+        HYB_CUDA(cudaGetLastError());
+        ++launches;
+      }
       // pack the occupied slots on the device; only they travel to the host
       const uint64_t group_slots = table_control[0];
       const size_t compact_words = std::max<uint64_t>(group_slots, 1) * per_slot_words;
@@ -2453,7 +2672,7 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
             const double deviation = std::sqrt(m2 / (n - 1.0));
             std::memcpy(&group.accumulators[a], &deviation, sizeof(deviation));
           }
-          if ((function == HYB_AGG_MIN || function == HYB_AGG_MAX) && group.counts[a] > 0) {
+          if ((function == HYB_AGG_MIN || function == HYB_AGG_MAX) && group.counts[a] > 0 && input_types[a] != HYB_TYPE_STRING) {
             const bool integral = input_types[a] == HYB_TYPE_INT32 || input_types[a] == HYB_TYPE_INT64;
             if (integral) {
               group.accumulators[a] ^= 0x8000000000000000ull;
@@ -2590,7 +2809,9 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
           break;
         }
         default: {  // MIN / MAX in the column type
-          if (result_types[a] == HYB_TYPE_INT32) {
+          if (result_types[a] == HYB_TYPE_STRING) {
+            std::memcpy(out, &bits, 8);  // the hyb_dictionary_position string_extreme_kernel wrote
+          } else if (result_types[a] == HYB_TYPE_INT32) {
             const int32_t value = static_cast<int32_t>(static_cast<int64_t>(bits));
             std::memcpy(out, &value, sizeof(value));
           } else if (result_types[a] == HYB_TYPE_INT64) {
@@ -3070,6 +3291,22 @@ int hyb_aggregate_hash_distributed(hyb_context* context, hyb_peer_group_t group_
   PeerGroup* group = find_peer_group(context, group_handle);
   HYB_CHECK(group, HYB_ERR_NOT_FOUND, "unknown peer group handle");
   HYB_CHECK(group->connected || group->world == 1, HYB_ERR_INVALID, "peer group is not connected");
+  if (const Table* table = find_table(context, query->table)) {
+    for (uint32_t a = 0; a < query->aggregate_count; ++a) {
+      // Every shard would rank its strings on its own, and ANY names rows of the shard: like COUNT(DISTINCT), all ranks
+      // decline before any exchange.
+      const auto& def = query->aggregates[a];
+      if (def.function == HYB_AGG_COUNT_STAR) continue;  // no argument; its nodes are never read
+      HYB_CHECK(def.node_count <= HYB_MAX_EXPR_NODES, HYB_ERR_INVALID, "bad expression length");
+      bool string_argument = false;
+      for (uint32_t n = 0; n < def.node_count; ++n) {
+        string_argument |= def.nodes[n].op == HYB_EXPR_COLUMN && def.nodes[n].column_id < table->column_count &&
+                           table->column_types[def.nodes[n].column_id] == HYB_TYPE_STRING;
+      }
+      HYB_CHECK(def.function != HYB_AGG_ANY && !string_argument, HYB_ERR_UNSUPPORTED,
+                "distributed ANY and aggregates over string columns run on the CPU operator");
+    }
+  }
   group->stats = hyb_distributed_stats{};
   for (int event = 0; event < 5; ++event) HYB_CUDA(cudaEventRecord(group->events[event], context->stream));
   const AggregateExchange exchange{group, chunk_id_base, position_base};
@@ -3110,6 +3347,9 @@ int hyb_aggregate_result_values(hyb_context* context, hyb_aggregate_result_t han
   HYB_CHECK(result, HYB_ERR_NOT_FOUND, "unknown aggregate result handle");
   HYB_CHECK(aggregate_index < result->columns.size(), HYB_ERR_INVALID, "aggregate_index out of range");
   const auto& column = result->columns[aggregate_index];
+  HYB_CHECK(!column.is_any, HYB_ERR_INVALID,
+            "aggregate " + std::to_string(aggregate_index) +
+                " is ANY: its values are the column at the representative RowIDs (hyb_aggregate_result_row_ids)");
   if (out_values && !column.values.empty()) std::memcpy(out_values, column.values.data(), column.values.size());
   if (out_nulls && !column.nulls.empty()) std::memcpy(out_nulls, column.nulls.data(), column.nulls.size());
   if (out_value_type) *out_value_type = column.value_type;
@@ -3230,6 +3470,9 @@ int hyb_aggregate_result_top_k(hyb_context* context, hyb_aggregate_result_t hand
   auto* result = find_aggregate_result(context, handle);
   HYB_CHECK(result, HYB_ERR_NOT_FOUND, "unknown aggregate result handle");
   HYB_CHECK(aggregate_index < result->columns.size(), HYB_ERR_INVALID, "aggregate_index out of range");
+  HYB_CHECK(!result->columns[aggregate_index].is_any, HYB_ERR_INVALID, "ANY has no values to sort by");
+  HYB_CHECK(result->columns[aggregate_index].value_type != HYB_TYPE_STRING, HYB_ERR_UNSUPPORTED,
+            "sorting by a string aggregate runs on the CPU operator");
   const uint64_t groups = result->group_count;
   HYB_CHECK(groups < 0xFFFFFFF0ull, HYB_ERR_UNSUPPORTED, "too many groups");
   *out_count = static_cast<uint32_t>(std::min<uint64_t>(k, groups));

@@ -607,6 +607,31 @@ int hyb_binary_table_column_translation(const hyb_binary_table* table, uint32_t 
   return HYB_OK;
 }
 
+int hyb_binary_table_string_order_ranks(const hyb_binary_table* table, uint32_t column, uint32_t* out_ranks,
+                                        uint32_t* inout_count) {
+  HYB_CHECK(table && inout_count, HYB_ERR_INVALID, "NULL argument");
+  const size_t columns = table->column_types.size();
+  HYB_CHECK(column < columns && table->column_types[column] == HYB_TYPE_STRING, HYB_ERR_INVALID, "not a string column");
+  std::vector<LikeDictionary> dictionaries(table->chunk_rows.size());
+  uint64_t words = 0;
+  for (size_t chunk = 0; chunk < table->chunk_rows.size(); ++chunk) {
+    const auto& dictionary = table->string_dictionaries[chunk * columns + column];
+    const uint32_t size = dictionary.offsets.empty() ? 0 : static_cast<uint32_t>(dictionary.offsets.size() - 1);
+    // chars.data() is NULL for a dictionary that holds only the empty string
+    dictionaries[chunk] = LikeDictionary{dictionary.chars.data(), dictionary.offsets.data(), size};
+    words += size;
+  }
+  HYB_CHECK(words <= UINT32_MAX, HYB_ERR_INVALID, "ranks exceed 2^32 words");
+  if (!out_ranks) {
+    *inout_count = static_cast<uint32_t>(words);
+    return HYB_OK;
+  }
+  HYB_CHECK(*inout_count >= words, HYB_ERR_INVALID, "out_ranks holds fewer words than the ranks need");
+  HYB_TRY(order_rank_dictionaries(dictionaries.data(), dictionaries.size(), out_ranks, nullptr));
+  *inout_count = static_cast<uint32_t>(words);
+  return HYB_OK;
+}
+
 int hyb_table_upload_binary(hyb_context* context, const hyb_binary_table* table, hyb_table_t* out_table) {
   HYB_CHECK(context && table && out_table, HYB_ERR_INVALID, "NULL argument");
   hyb_block_set_t block_set = 0;

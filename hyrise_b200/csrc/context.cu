@@ -100,6 +100,12 @@ Table::~Table() {
   for (auto& entry : d_tile_maps) table_free(owner, entry.second.first);
 }
 
+Table::StringColumnView::~StringColumnView() {
+  device_free(owner, d_segments);
+  device_free(owner, d_words);
+  device_free(owner, d_first_entry);
+}
+
 PosList::~PosList() {
   device_free(owner, d_row_ids);
   device_free(owner, d_chunk_end);
@@ -229,6 +235,7 @@ int sync_table_descriptors(hyb_context* context, Table* table) {
   table->d_tile_maps.clear();
   table->key_bounds.clear();
   table->plan_memo.clear();
+  table->string_views.clear();
   table->dirty = false;
   return HYB_OK;
 }

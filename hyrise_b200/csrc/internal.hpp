@@ -107,6 +107,20 @@ struct Table {
   // bytes per launch ...), keyed by the shape's signature: like the reference's physical-plan cache it spares a repeated
   // query the O(chunks x columns) analysis. Dropped with the key bounds whenever chunks change.
   std::map<std::string, std::shared_ptr<void>> plan_memo;
+  // A string dictionary column seen by AggregateHash as an INT32 dictionary column: same attribute vectors, vector types,
+  // bit widths and NULL value-IDs, with per-entry words as dictionaries. `ordered`: the words are the column's order ranks
+  // (hyb_table_set_string_order) and `d_first_entry[rank]` = chunk_id << 32 | value_id of the first entry (in chunk order)
+  // that holds the rank. Otherwise the words are zeros, which is all COUNT needs. Dropped with the key bounds.
+  struct StringColumnView {
+    hyb_context* owner = nullptr;
+    DevSegment* d_segments = nullptr;           // chunk_count descriptors
+    uint32_t* d_words = nullptr;
+    unsigned long long* d_first_entry = nullptr;
+    uint64_t word_count = 0;                    // rank words: the sum of the dictionary sizes
+    bool ordered = false;
+    ~StringColumnView();
+  };
+  std::map<uint32_t, std::shared_ptr<StringColumnView>> string_views;
 
   uint32_t chunk_count() const { return static_cast<uint32_t>(chunk_rows.size()); }
   uint64_t row_count() const { return chunk_row_start.empty() ? 0 : chunk_row_start.back(); }
@@ -157,6 +171,7 @@ struct AggregateColumn {
   int32_t value_type = 0;             // hyb_data_type of the result
   std::vector<uint8_t> values;        // group_count * element size
   std::vector<uint8_t> nulls;         // group_count
+  bool is_any = false;                // ANY: no values; the column at the representative RowIDs (value_type = its type)
 };
 
 struct AggregateResult {
@@ -281,6 +296,10 @@ int like_match_dictionaries(const char* pattern, uint64_t pattern_length, int32_
 // hyb_dictionary_translate (translate.cu): right_in_left of one chunk, right.count words, for two sorted unique
 // dictionaries in the layout above.
 int translate_dictionary(const LikeDictionary& left, const LikeDictionary& right, uint32_t* out_words);
+// hyb_dictionary_order_ranks (translate.cu): dense ranks of every entry among the distinct strings of all dictionaries,
+// in dictionary order.
+int order_rank_dictionaries(const LikeDictionary* dictionaries, size_t dictionary_count, uint32_t* out_ranks,
+                            uint32_t* out_distinct_count);
 // hyb_in_dictionary_matches (in_list.cu) over several dictionaries, their bitmaps concatenated in out_words.
 int in_match_dictionaries(int32_t condition, const LikeDictionary& elements, const LikeDictionary* dictionaries,
                           size_t dictionary_count, uint32_t* out_words, uint64_t* out_match_count);

@@ -16,6 +16,8 @@ from .capi import check
 from .storage import NUMPY_TYPES, Table, TableViewHolder
 
 ROW_ID_DTYPE = np.dtype([("chunk_id", np.uint32), ("chunk_offset", np.uint32)])
+# hyb_dictionary_position: a string MIN / MAX result, entry value_id of chunk chunk_id's dictionary
+POSITION_DTYPE = np.dtype([("chunk_id", np.uint32), ("value_id", np.uint32)])
 
 
 @dataclass
@@ -311,10 +313,18 @@ class AggregateOutput:
     group_count: int
     used_immediate_keys: bool
     row_ids: np.ndarray
-    values: list[np.ndarray]
-    nulls: list[np.ndarray]
-    value_types: list[int]
+    values: list[np.ndarray | None]  # POSITION_DTYPE for string MIN / MAX; None for ANY (the column at row_ids)
+    nulls: list[np.ndarray | None]
+    value_types: list[int]           # ANY: the column's type
     result_handle: int = 0   # != 0: the device-side result is still alive (aggregate_hash(..., keep_result=True))
+
+
+def string_values(host_table: Table, column_id: int, positions: np.ndarray, nulls: np.ndarray) -> list:
+    """The strings a string MIN / MAX result names (bytes per group, None for NULL), read from the host table's
+    dictionaries."""
+    return [None if null else bytes(host_table.chunks[int(position["chunk_id"])].segments[column_id]
+                                    .string_dictionary[int(position["value_id"])])
+            for position, null in zip(positions, nulls)]
 
 
 class DevicePeerGroup:
@@ -492,7 +502,17 @@ class DeviceContext:
     def free_aggregate_result(self, result_handle: int) -> None:
         check(self.lib.hyb_aggregate_result_free(self.ptr, result_handle))
 
-    def _collect_aggregate(self, handle: int, aggregate_count: int, keep_result: bool = False) -> AggregateOutput:
+    def set_string_order(self, table: DeviceTable, column_id: int, ranks: np.ndarray | None = None) -> None:
+        """hyb_table_set_string_order: attach the order ranks MIN / MAX over a string column need; computed from the host
+        table's dictionaries unless `ranks` is given (e.g. NativeBinaryTable.string_order_ranks)."""
+        if ranks is None:
+            ranks = table.host_table.string_order_ranks(column_id)
+        ranks = np.ascontiguousarray(ranks, dtype=np.uint32)
+        check(self.lib.hyb_table_set_string_order(self.ptr, table.handle, column_id,
+                                                  ranks.ctypes.data_as(C.POINTER(C.c_uint32)), len(ranks)))
+
+    def _collect_aggregate(self, handle: int, aggregate_count: int, keep_result: bool = False,
+                           any_types: dict | None = None) -> AggregateOutput:
         try:
             groups, immediate = C.c_uint64(), C.c_int32()
             check(self.lib.hyb_aggregate_result_info(self.ptr, handle, C.byref(groups), C.byref(immediate)))
@@ -501,12 +521,17 @@ class DeviceContext:
             check(self.lib.hyb_aggregate_result_row_ids(self.ptr, handle, row_ids.ctypes.data))
             values, nulls, types = [], [], []
             for index in range(aggregate_count):
+                if any_types and index in any_types:
+                    values.append(None)
+                    nulls.append(None)
+                    types.append(any_types[index])
+                    continue
                 raw = np.zeros(max(count, 1), dtype=np.uint64)
                 null = np.zeros(max(count, 1), dtype=np.uint8)
                 value_type = C.c_int32()
                 check(self.lib.hyb_aggregate_result_values(self.ptr, handle, index, raw.ctypes.data, null.ctypes.data,
                                                            C.byref(value_type)))
-                dtype = NUMPY_TYPES[value_type.value]
+                dtype = POSITION_DTYPE if value_type.value == capi.TYPE_STRING else NUMPY_TYPES[value_type.value]
                 values.append(raw.view(np.uint8)[: count * np.dtype(dtype).itemsize].view(dtype).copy())
                 nulls.append(null[:count].astype(bool))
                 types.append(value_type.value)
@@ -524,7 +549,10 @@ class DeviceContext:
         handle = C.c_uint64()
         check(self.lib.hyb_aggregate_hash(self.ptr, C.byref(query), C.byref(handle)))
         del keepalive
-        return self._collect_aggregate(handle.value, len(aggregates), keep_result)
+        definitions = table.host_table.column_definitions
+        any_types = {index: definitions[aggregate.expression.nodes[0][1]].data_type
+                     for index, aggregate in enumerate(aggregates) if aggregate.function == capi.AGG_ANY}
+        return self._collect_aggregate(handle.value, len(aggregates), keep_result, any_types)
 
     def last_stats(self) -> capi.OperatorStats:
         stats = capi.OperatorStats()

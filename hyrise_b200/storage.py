@@ -177,6 +177,15 @@ class StringKeyRegistry:
         return out
 
 
+def dictionary_order_ranks(dictionaries) -> np.ndarray:
+    """Restatement of hyb_dictionary_order_ranks: the dense rank of every entry of every dictionary (sequences of bytes)
+    among the distinct strings of all of them, as Python orders bytes (unsigned, a proper prefix first), dictionary
+    after dictionary."""
+    dictionaries = [[bytes(entry) for entry in dictionary] for dictionary in dictionaries]
+    rank = {value: index for index, value in enumerate(sorted({entry for dictionary in dictionaries for entry in dictionary}))}
+    return np.array([rank[entry] for dictionary in dictionaries for entry in dictionary], dtype=np.uint32)
+
+
 def make_value_segment(values: np.ndarray, nulls: np.ndarray | None, data_type: int) -> Segment:
     if data_type == capi.TYPE_STRING:
         raise capi.UnsupportedOnDevice(capi.HYB_ERR_UNSUPPORTED, "unencoded string segments stay on the CPU")
@@ -387,6 +396,11 @@ class Table:
                                            chunk.segments[right_column_id].string_dictionary)
                  for chunk in self.chunks]
         return np.concatenate(words) if words else np.zeros(0, dtype=np.uint32)
+
+    def string_order_ranks(self, column_id: int) -> np.ndarray:
+        """hyb_table_set_string_order's words for a string column: every dictionary entry's dense rank among the column's
+        distinct strings, chunk after chunk (dictionary_order_ranks over the chunks' dictionaries)."""
+        return dictionary_order_ranks([chunk.segments[column_id].string_dictionary for chunk in self.chunks])
 
     def column_values(self, column_id: int) -> tuple[np.ndarray, np.ndarray]:
         """Decoded values and null mask of a whole column (host side)."""

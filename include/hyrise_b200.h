@@ -134,7 +134,8 @@ typedef enum hyb_aggregate_function {
   HYB_AGG_COUNT_STAR = 5, /* COUNT(*): INVALID_COLUMN_ID argument in the reference */
   HYB_AGG_COUNT_DISTINCT = 6,     /* over a STRING column: a bare column whose segments carry dictionary_codes */
   HYB_AGG_STDDEV_SAMP = 7,        /* numeric arguments only (a STRING argument is HYB_ERR_INVALID) */
-  HYB_AGG_ANY = 8                 /* pseudo aggregate: handled like a group-by column by the shim */
+  HYB_AGG_ANY = 8                 /* pseudo aggregate: a single column, any type; no values (hyb_aggregate_result_values
+                                     returns HYB_ERR_INVALID): the shim writes the column at the representative RowIDs */
 } hyb_aggregate_function;
 
 /* A typed scalar, already losslessly cast to the column type by the shim (utils/lossless_predicate_cast.hpp:20-60). */
@@ -293,6 +294,17 @@ int hyb_table_upload_binary(hyb_context* context, const hyb_binary_table* table,
 int hyb_table_info(hyb_context* context, hyb_table_t table, uint32_t* out_chunk_count, uint32_t* out_column_count,
                    uint64_t* out_row_count, uint64_t* out_device_bytes);
 
+/*
+ * Attach the order ranks of a STRING dictionary column (hyb_dictionary_order_ranks over its dictionaries): `count` words,
+ * one per dictionary entry, chunk after chunk. AggregateHash needs them for MIN / MAX over the column (HYB_ERR_UNSUPPORTED
+ * without), and reads them as the dictionaries of an INT32 dictionary column with the same value-IDs. HYB_ERR_INVALID:
+ * not a string dictionary column, `count` != the sum of the dictionary sizes, words not strictly increasing within a
+ * chunk, or a word of 2^31 or more. Appending a chunk drops the ranks. Ranks that disagree across chunks (different
+ * words for one string) give wrong MIN / MAX results; they cannot be checked without the strings.
+ */
+int hyb_table_set_string_order(hyb_context* context, hyb_table_t table, uint32_t column, const uint32_t* ranks,
+                               uint64_t count);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * TableScan
  * ---------------------------------------------------------------------------------------------------------------- */
@@ -403,6 +415,23 @@ int hyb_table_scan_columns(hyb_context* context, hyb_table_t table, const hyb_co
 int hyb_dictionary_translate(const char* left_chars, const uint64_t* left_offsets, uint32_t left_count,
                              const char* right_chars, const uint64_t* right_offsets, uint32_t right_count,
                              uint32_t* out_words);
+
+/*
+ * Order ranks of a string column (host only, no GPU): every entry of `dictionary_count` sorted dictionaries (entry i of
+ * dictionary d = chars[d][offsets[d][i] .. offsets[d][i + 1]), the layout of hyb_dictionary_translate; chars[d] may be
+ * NULL when every entry is empty) gets its dense rank among the distinct strings of all of them, by bytewise comparison
+ * (unsigned chars; a proper prefix sorts first). Equal strings share a rank. out_ranks receives the sum of counts[] words,
+ * dictionary after dictionary; out_distinct_count (optional) the number of distinct strings. One k-way merge.
+ * HYB_ERR_INVALID: a dictionary that is not strictly increasing; HYB_ERR_UNSUPPORTED: 2^31 or more distinct strings.
+ */
+int hyb_dictionary_order_ranks(uint32_t dictionary_count, const char* const* chars, const uint64_t* const* offsets,
+                               const uint32_t* counts, uint32_t* out_ranks, uint32_t* out_distinct_count);
+
+/* hyb_dictionary_order_ranks over every chunk's dictionary of a string column of a parsed binary table, in chunk order.
+ * out_ranks == NULL: only *inout_count is set, to the number of words needed; otherwise *inout_count must be at least
+ * that. */
+int hyb_binary_table_string_order_ranks(const hyb_binary_table* table, uint32_t column, uint32_t* out_ranks,
+                                        uint32_t* inout_count);
 
 /*
  * <column> [NOT] IN (<literal>, ...): ExpressionEvaluator::_evaluate_in_expression (expression_evaluator.cpp:404-511) on a
@@ -613,7 +642,8 @@ int hyb_join_hash_distributed(hyb_context* context, hyb_peer_group_t group, cons
  * Representative RowIDs refer to the global table (chunk ids shifted by chunk_id_base); position_base = number of rows of
  * the global table before this rank's shard (first-appearance order across ranks).
  * COUNT(DISTINCT) and STDDEV_SAMP return HYB_ERR_UNSUPPORTED before any exchange (their partial states do not merge
- * through the blocks); every rank sees the same query, so all ranks decline together.
+ * through the blocks); so do ANY and any aggregate over a string column (each shard would rank its own strings). Every
+ * rank sees the same query, so all ranks decline together.
  */
 int hyb_aggregate_hash_distributed(hyb_context* context, hyb_peer_group_t group, const struct hyb_aggregate_query* query,
                                    uint32_t chunk_id_base, uint64_t position_base, hyb_aggregate_result_t* out_result);
@@ -704,12 +734,24 @@ int hyb_aggregate_result_row_ids(hyb_context* context, hyb_aggregate_result_t re
  * `out_values` receives group_count elements of that type (8 bytes for int64/double, 4 for int32/float); out_value_type
  * tells which. out_nulls (optional) gets 1 where the reference writes NULL (aggregate_count == 0).
  *
+ * Over a STRING column, as a bare column only (a string expression: HYB_ERR_UNSUPPORTED):
+ *   COUNT -> int64, the non-NULL rows (value-ID != dictionary size); takes the general kernel.
+ *   MIN / MAX -> out_value_type HYB_TYPE_STRING: one hyb_dictionary_position per group, the entry of the table's
+ *     dictionaries holding the smallest / largest string (bytewise, as char_traits<char>::compare), NULL when the group
+ *     has no non-NULL value. Needs hyb_table_set_string_order on the column; runs on the general kernel.
+ * ANY -> HYB_ERR_INVALID here: its values are the column at hyb_aggregate_result_row_ids. ANY never changes the kernel
+ * or the groups of the other aggregates; an all-ANY query returns what the query without aggregates returns.
+ *
  * COUNT(DISTINCT) over a STRING column is accepted as a bare column whose DICTIONARY segments all carry
  * dictionary_codes (equal codes <=> equal strings); otherwise, and for a string expression, HYB_ERR_UNSUPPORTED.
  * STDDEV_SAMP uses the corrected two-pass method (a second sweep over the same rows), not Welford's sequential update:
  * results agree with the reference to rounding, and a group of equal int32 / float values gives exactly 0.0 while it
  * holds fewer than 2^22 / 2^29 rows.
  */
+typedef struct hyb_dictionary_position { /* a string MIN / MAX: entry value_id of chunk chunk_id's dictionary */
+  uint32_t chunk_id;
+  uint32_t value_id;
+} hyb_dictionary_position;
 int hyb_aggregate_result_values(hyb_context* context, hyb_aggregate_result_t result, uint32_t aggregate_index,
                                 void* out_values, uint8_t* out_nulls, int32_t* out_value_type);
 int hyb_aggregate_result_free(hyb_context* context, hyb_aggregate_result_t result);

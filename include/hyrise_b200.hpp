@@ -78,7 +78,8 @@ enum class WindowFunction : int32_t {
   Count = HYB_AGG_COUNT,
   CountStar = HYB_AGG_COUNT_STAR,
   CountDistinct = HYB_AGG_COUNT_DISTINCT,
-  StandardDeviationSample = HYB_AGG_STDDEV_SAMP
+  StandardDeviationSample = HYB_AGG_STDDEV_SAMP,
+  Any = HYB_AGG_ANY  // one column, no values: the column at AggregateOutput::group_row_ids()
 };
 
 // HYB_ERR_UNSUPPORTED: the caller runs the reference's CPU operator instead (IN scans, string join keys, ...).
@@ -183,6 +184,24 @@ class BinaryTable {
     check(hyb_binary_table_column_translation(_table, left_column, right_column, translation.data(), &words));
     return translation;
   }
+  // The order ranks of a string column (hyb_binary_table_string_order_ranks): DeviceTable::set_string_order's words
+  std::vector<uint32_t> string_order_ranks(uint32_t column) const {
+    uint32_t words = 0;
+    check(hyb_binary_table_string_order_ranks(_table, column, nullptr, &words));
+    std::vector<uint32_t> ranks(std::max<uint32_t>(words, 1));
+    check(hyb_binary_table_string_order_ranks(_table, column, ranks.data(), &words));
+    ranks.resize(words);
+    return ranks;
+  }
+  // One dictionary entry of a string column (a string MIN / MAX result names one).
+  std::string dictionary_entry(uint32_t chunk, uint32_t column, uint32_t value_id) const {
+    const char* chars = nullptr;
+    const uint64_t* offsets = nullptr;
+    uint32_t count = 0;
+    check(hyb_binary_table_string_dictionary(_table, chunk, column, &chars, &offsets, &count));
+    if (value_id >= count) throw std::out_of_range("value-ID outside the dictionary");
+    return std::string(chars ? chars + offsets[value_id] : "", offsets[value_id + 1] - offsets[value_id]);
+  }
 
  private:
   hyb_binary_table* _table = nullptr;
@@ -202,6 +221,10 @@ class DeviceTable {
   DeviceTable& operator=(const DeviceTable&) = delete;
   hyb_table_t handle() const { return _handle; }
   const std::shared_ptr<DeviceContext>& context() const { return _context; }
+  // Attach the order ranks MIN / MAX over a string column need (dropped when chunks are appended).
+  void set_string_order(uint32_t column, const std::vector<uint32_t>& ranks) {
+    check(hyb_table_set_string_order(_context->get(), _handle, column, ranks.data(), ranks.size()));
+  }
   uint64_t row_count() const {
     uint64_t rows = 0;
     check(hyb_table_info(_context->get(), _handle, nullptr, nullptr, &rows, nullptr));
@@ -695,6 +718,20 @@ class AggregateOutput {
     }
     if (value_type) *value_type = type;
     return {std::move(out), std::move(nulls)};
+  }
+  // A string MIN / MAX: per group the string (std::nullopt for NULL), read from the table the aggregate ran on.
+  std::vector<std::optional<std::string>> strings(uint32_t aggregate_index, const BinaryTable& table, uint32_t column) const {
+    const auto groups = group_count();
+    std::vector<hyb_dictionary_position> positions(groups);
+    std::vector<uint8_t> nulls(groups);
+    int32_t type = 0;
+    if (groups) check(hyb_aggregate_result_values(_context->get(), _handle, aggregate_index, positions.data(), nulls.data(), &type));
+    if (groups && type != HYB_TYPE_STRING) throw std::invalid_argument("not a string aggregate");
+    std::vector<std::optional<std::string>> out(groups);
+    for (uint64_t g = 0; g < groups; ++g) {
+      if (!nulls[g]) out[g] = table.dictionary_entry(positions[g].chunk_id, column, positions[g].value_id);
+    }
+    return out;
   }
 
  private:

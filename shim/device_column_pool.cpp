@@ -169,7 +169,59 @@ bool DeviceColumnPool::upload(const std::shared_ptr<const Table>& table) {
     const auto status = hyb_table_append_chunk(_context, entry.handle, descs.data());  // copies every buffer; borrowed for the call
     Assert(status == HYB_OK, hyb_last_error());
     entry.uploaded_chunks = ChunkID{static_cast<uint32_t>(chunk_id) + 1};
+    entry.ordered.assign(column_count, false);  // the library dropped the order ranks with the new chunk
   }
+  return true;
+}
+
+bool DeviceColumnPool::ensure_string_order(const std::shared_ptr<const Table>& table, ColumnID column_id) {
+  if (table->column_data_type(column_id) != DataType::String) {
+    return false;
+  }
+  const auto lock = std::lock_guard<std::mutex>{_mutex};
+  const auto iter = _entries.find(table.get());
+  if (iter == _entries.end() || iter->second.uploaded_chunks != table->chunk_count()) {
+    return false;
+  }
+  auto& entry = iter->second;
+  entry.ordered.resize(table->column_count(), false);
+  if (entry.ordered[column_id]) {
+    return true;
+  }
+  // the dictionaries of the uploaded chunks in the layout of hyb_dictionary_order_ranks (one k-way merge on the host)
+  const auto chunk_count = table->chunk_count();
+  auto chars = std::vector<std::string>(chunk_count);
+  auto offsets = std::vector<std::vector<uint64_t>>(chunk_count);
+  auto char_pointers = std::vector<const char*>(chunk_count);
+  auto offset_pointers = std::vector<const uint64_t*>(chunk_count);
+  auto counts = std::vector<uint32_t>(chunk_count);
+  auto total = uint64_t{0};
+  for (auto chunk_id = ChunkID{0}; chunk_id < chunk_count; ++chunk_id) {
+    const auto segment =
+        std::dynamic_pointer_cast<const DictionarySegment<pmr_string>>(table->get_chunk(chunk_id)->get_segment(column_id));
+    if (!segment) {
+      return false;
+    }
+    const auto& dictionary = *segment->dictionary();
+    offsets[chunk_id].push_back(0);
+    for (const auto& value : dictionary) {
+      chars[chunk_id].append(value.data(), value.size());
+      offsets[chunk_id].push_back(chars[chunk_id].size());
+    }
+    char_pointers[chunk_id] = chars[chunk_id].data();
+    offset_pointers[chunk_id] = offsets[chunk_id].data();
+    counts[chunk_id] = static_cast<uint32_t>(dictionary.size());
+    total += dictionary.size();
+  }
+  auto ranks = std::vector<uint32_t>(total);
+  const auto status = hyb_dictionary_order_ranks(static_cast<uint32_t>(chunk_count), char_pointers.data(), offset_pointers.data(),
+                                                 counts.data(), ranks.data(), nullptr);
+  if (status == HYB_ERR_UNSUPPORTED) {
+    return false;
+  }
+  Assert(status == HYB_OK, hyb_last_error());
+  Assert(hyb_table_set_string_order(_context, entry.handle, column_id, ranks.data(), total) == HYB_OK, hyb_last_error());
+  entry.ordered[column_id] = true;
   return true;
 }
 

@@ -26,11 +26,16 @@ class DeviceColumnPool {
     hyb_table_t handle{0};
     ChunkID uploaded_chunks{0};
     std::vector<std::unordered_map<std::string, uint64_t>> string_ids;  // per column: group-by codes of long strings
+    std::vector<bool> ordered;  // per column: order ranks attached (hyb_table_set_string_order; appending drops them)
   };
 
   // The device table of a stored table, or of the single stored table all ReferenceSegments of `table` point to (then
   // `out_referenced` is that table); nullptr if there is none.
   const Entry* find(const std::shared_ptr<const Table>& table, std::shared_ptr<const Table>* out_referenced = nullptr) const;
+
+  // Computes and attaches the order ranks string MIN / MAX need, once per uploaded string column (after new chunks, again).
+  // false: the column is no string dictionary column of an uploaded table, or the ranks do not fit (2^31 strings).
+  bool ensure_string_order(const std::shared_ptr<const Table>& table, ColumnID column_id);
 
   hyb_context* context() const {
     return _context;

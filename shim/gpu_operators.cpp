@@ -473,8 +473,12 @@ std::shared_ptr<const Table> try_gpu_aggregate_hash(const std::shared_ptr<const 
       case WindowFunction::StandardDeviationSample:
         definition.function = HYB_AGG_STDDEV_SAMP;
         break;
+      case WindowFunction::Any:
+        // no accumulator: the column at the representative RowIDs (DependentGroupByReductionRule, SELECT DISTINCT)
+        definition.function = HYB_AGG_ANY;
+        break;
       default:
-        return nullptr;  // Any (a pseudo aggregate the caller handles) and the window functions: the CPU operator
+        return nullptr;  // the window functions: the CPU operator
     }
     const auto column = std::dynamic_pointer_cast<const PQPColumnExpression>(aggregate.argument());
     if (aggregate.window_function == WindowFunction::Count && (!column || column->column_id == INVALID_COLUMN_ID)) {
@@ -489,6 +493,12 @@ std::shared_ptr<const Table> try_gpu_aggregate_hash(const std::shared_ptr<const 
     nodes[index].column_id = column->column_id;
     definition.nodes = &nodes[index];
     definition.node_count = 1;
+    const auto string_extreme = (aggregate.window_function == WindowFunction::Min ||
+                                 aggregate.window_function == WindowFunction::Max) &&
+                                in_table->column_data_type(column->column_id) == DataType::String;
+    if (string_extreme && !pool->ensure_string_order(in_table, column->column_id)) {
+      return nullptr;
+    }
   }
   auto groupby = std::vector<uint32_t>(groupby_column_ids.begin(), groupby_column_ids.end());
   auto query = hyb_aggregate_query{};
@@ -500,7 +510,7 @@ std::shared_ptr<const Table> try_gpu_aggregate_hash(const std::shared_ptr<const 
   auto result = hyb_aggregate_result_t{};
   const auto status = hyb_aggregate_hash(pool->context(), &query, &result);
   if (status == HYB_ERR_UNSUPPORTED) {
-    return nullptr;  // string aggregates other than COUNT(DISTINCT) of a dictionary column
+    return nullptr;  // SUM / AVG / expressions of strings, more aggregates or group-by columns than the device takes
   }
   Assert(status == HYB_OK, hyb_last_error());
   // Output: group-by columns as ReferenceSegments over the representative RowIDs (write_groupby_output, aggregate_hash.cpp:
@@ -519,9 +529,38 @@ std::shared_ptr<const Table> try_gpu_aggregate_hash(const std::shared_ptr<const 
   }
   for (auto index = size_t{0}; index < aggregates.size(); ++index) {
     const auto result_type = aggregates[index]->data_type();  // WindowFunctionTraits (window_function_traits.hpp:14-77)
+    if (aggregates[index]->window_function == WindowFunction::Any) {
+      // write_groupby_output (aggregate_hash.cpp:421-537): ANY columns are ReferenceSegments like the group-by columns
+      const auto column_id = std::static_pointer_cast<const PQPColumnExpression>(aggregates[index]->argument())->column_id;
+      segments.emplace_back(std::make_shared<ReferenceSegment>(in_table, column_id, row_ids));
+      output_definitions.emplace_back(aggregates[index]->as_column_name(), result_type, true);
+      continue;
+    }
     resolve_data_type(result_type, [&](const auto type) {
       using AggregateType = typename decltype(type)::type;
-      if constexpr (!std::is_same_v<AggregateType, pmr_string>) {
+      if constexpr (std::is_same_v<AggregateType, pmr_string>) {
+        // MIN / MAX of a string column: one dictionary position per group, the string read from the stored table's
+        // DictionarySegment (its dictionary entry); NULL groups stay empty strings under their NULL flag
+        auto positions = std::vector<hyb_dictionary_position>(group_count);
+        auto null_bytes = std::vector<uint8_t>(group_count);
+        auto value_type = int32_t{0};
+        Assert(hyb_aggregate_result_values(pool->context(), result, static_cast<uint32_t>(index), positions.data(),
+                                           null_bytes.data(), &value_type) == HYB_OK,
+               hyb_last_error());
+        Assert(value_type == HYB_TYPE_STRING, "result type mismatch between the shim and the library");
+        const auto column_id = std::static_pointer_cast<const PQPColumnExpression>(aggregates[index]->argument())->column_id;
+        auto values = pmr_vector<pmr_string>(group_count);
+        for (auto group = uint64_t{0}; group < group_count; ++group) {
+          if (null_bytes[group]) {
+            continue;
+          }
+          const auto segment = std::static_pointer_cast<const DictionarySegment<pmr_string>>(
+              in_table->get_chunk(ChunkID{positions[group].chunk_id})->get_segment(column_id));
+          values[group] = (*segment->dictionary())[positions[group].value_id];
+        }
+        auto nulls = pmr_vector<bool>(null_bytes.begin(), null_bytes.end());
+        segments.emplace_back(std::make_shared<ValueSegment<pmr_string>>(std::move(values), std::move(nulls)));
+      } else {
         auto values = pmr_vector<AggregateType>(group_count);
         auto null_bytes = std::vector<uint8_t>(group_count);
         auto value_type = int32_t{0};
