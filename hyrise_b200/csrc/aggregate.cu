@@ -2018,11 +2018,7 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
   const TestProgram* tree_program = tree ? tree->device : nullptr;
 
   uint64_t position_count = table->row_count();
-  if (filter) {
-    HYB_CUDA(cudaStreamSynchronize(stream));
-    HYB_CUDA(cudaMemcpy(&position_count, filter->d_chunk_end + filter->chunk_count, sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    if (position_count == ~uint64_t{0}) position_count = 0;
-  }
+  if (filter) HYB_TRY(pos_list_total(context, filter, &position_count));
 
   std::vector<HostGroup> groups;
   bool done = false;

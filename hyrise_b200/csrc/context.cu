@@ -127,6 +127,14 @@ PosList* find_pos_list(hyb_context* context, hyb_pos_list_t handle) {
   return it == context->pos_lists.end() ? nullptr : it->second.get();
 }
 
+int pos_list_total(hyb_context* context, const PosList* list, uint64_t* out_rows) {
+  HYB_CUDA(cudaStreamSynchronize(context->stream));
+  HYB_CUDA(cudaMemcpy(out_rows, list->d_chunk_end + list->chunk_count, sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  // a scan over a table without rows launches no tile: its total stays at the "unset" fill
+  if (*out_rows == ~uint64_t{0}) *out_rows = 0;
+  return HYB_OK;
+}
+
 static size_t cache_rounded_size(size_t bytes) {
   if (bytes <= 512) return 512;
   if (bytes >= (size_t{1} << 20)) return (bytes + (size_t{1} << 20) - 1) & ~((size_t{1} << 20) - 1);  // 1 MiB steps

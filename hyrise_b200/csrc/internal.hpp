@@ -325,6 +325,8 @@ class DeviceGuard {
 
 Table* find_table(hyb_context* context, hyb_table_t handle);
 PosList* find_pos_list(hyb_context* context, hyb_pos_list_t handle);
+// Rows in the list (synchronises the stream): d_chunk_end[chunk_count], with the "unset" fill of an empty scan read as 0.
+int pos_list_total(hyb_context* context, const PosList* list, uint64_t* out_rows);
 // Make the table's device descriptor arrays current (call with context->mutex held).
 int sync_table_descriptors(hyb_context* context, Table* table);
 // Device tile map: tiles of `tile_rows` rows never straddle a chunk; entry t = {chunk, first row | last-in-chunk << 31}.

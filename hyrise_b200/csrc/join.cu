@@ -1654,10 +1654,8 @@ static int prepare_side(hyb_context* context, const hyb_join_side* side, SideInf
     out->filter = find_pos_list(context, side->filter);
     HYB_CHECK(out->filter, HYB_ERR_NOT_FOUND, "unknown filter handle");
     HYB_CHECK(out->filter->table == side->table, HYB_ERR_INVALID, "filter belongs to a different table");
-    HYB_CUDA(cudaStreamSynchronize(context->stream));
     uint64_t count = 0;
-    HYB_CUDA(cudaMemcpy(&count, out->filter->d_chunk_end + out->filter->chunk_count, sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    if (count == ~uint64_t{0}) count = 0;
+    HYB_TRY(pos_list_total(context, out->filter, &count));
     out->positions = count;
     source.filter = out->filter->d_row_ids;
     source.null_key_zero = out->filter->ascending ? 0u : 1u;  // per-chunk scan lists are single-chunk PosLists

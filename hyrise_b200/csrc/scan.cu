@@ -24,6 +24,11 @@
 // (hyb_table_scan_in, the ExpressionEvaluator's _evaluate_in_expression on a literal list) uses them too, with InRows:
 // dictionary chunks scan a value-ID range or set built by in_prepare_kernel (numeric) or from the caller's dictionary
 // bitmaps (strings), Value / FrameOfReference chunks search the list's intervals (in_list.cuh).
+//
+// Host side: each of the five entry points (hyb_table_scan, _columns, _in, _expression, _expression_tests) checks and
+// prepares its predicate into a ScanPlan and the row evaluator's Extra, then ends in run_scan<Rows>: the result PosList,
+// the unfiltered launch (launch_unfiltered; only ColumnRows has the single-pass and bulk kernels) or the position-filtered
+// one, the operator stats and the handle. Every scratch block of a call belongs to a DeviceScratch.
 #include <algorithm>
 #include <cstddef>
 #include <cstdio>
@@ -1168,7 +1173,8 @@ static int prepare_bitmap_tests(hyb_context* context, Table* table, uint32_t col
   return HYB_OK;
 }
 
-// Shared by hyb_table_scan and the fused predicates of hyb_aggregate_hash: builds the per-chunk tests on the device.
+// Shared by hyb_table_scan and the fused predicates of hyb_aggregate_hash: builds the per-chunk tests on the device. The
+// caller owns both blocks on success; on failure neither is left allocated.
 int prepare_chunk_tests(hyb_context* context, Table* table, const hyb_scan_predicate* predicate, ChunkTest** out_tests,
                         void** out_bounds_scratch, uint64_t* out_uploaded_bytes) {
   *out_tests = nullptr;
@@ -1186,19 +1192,18 @@ int prepare_chunk_tests(hyb_context* context, Table* table, const hyb_scan_predi
     HYB_CHECK(data_type == HYB_TYPE_STRING, HYB_ERR_INVALID, "LIKE needs a string column");
     HYB_CHECK(predicate->value_id_bounds, HYB_ERR_INVALID,
               "LIKE scans need host-computed dictionary match bitmaps in value_id_bounds (hyb_like_dictionary_matches)");
-    void* tests = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(ChunkTest) * std::max<uint32_t>(chunk_count, 1), &tests));
+    DeviceScratch scratch(context);  // released to the caller on success
+    ChunkTest* tests = nullptr;
+    HYB_TRY(scratch.alloc_array(chunk_count, &tests));
+    void* bitmaps = nullptr;
     uint64_t words = 0;
     const int status = prepare_bitmap_tests(context, table, predicate->column_id, predicate->value_id_bounds, tests,
-                                            out_bounds_scratch, &words);
+                                            &bitmaps, &words);
+    scratch.adopt(bitmaps);
     if (out_uploaded_bytes) *out_uploaded_bytes = sizeof(uint32_t) * words;
-    if (status != HYB_OK) {
-      device_free(context, tests);
-      device_free(context, *out_bounds_scratch);
-      *out_bounds_scratch = nullptr;
-      return status;
-    }
-    *out_tests = static_cast<ChunkTest*>(tests);
+    HYB_TRY(status);
+    *out_bounds_scratch = scratch.release(bitmaps);
+    *out_tests = static_cast<ChunkTest*>(scratch.release(tests));
     return HYB_OK;
   }
   if (data_type == HYB_TYPE_STRING && needs_value) {
@@ -1210,26 +1215,29 @@ int prepare_chunk_tests(hyb_context* context, Table* table, const hyb_scan_predi
   device_predicate.data_type = data_type;
   device_predicate.lower = predicate->lower;
   device_predicate.upper = predicate->upper;
+  DeviceScratch scratch(context);  // released to the caller on success
+  uint32_t* bounds = nullptr;
   if (predicate->value_id_bounds && needs_value && chunk_count) {
     const bool between = predicate->condition >= HYB_PRED_BETWEEN_INCLUSIVE &&
                          predicate->condition <= HYB_PRED_BETWEEN_EXCLUSIVE;
-    const size_t bytes = sizeof(uint32_t) * size_t{chunk_count} * (between ? 4 : 2);
-    HYB_TRY(device_alloc(context, bytes, out_bounds_scratch));
-    HYB_CUDA(cudaMemcpyAsync(*out_bounds_scratch, predicate->value_id_bounds, bytes, cudaMemcpyHostToDevice,
+    const size_t words = size_t{chunk_count} * (between ? 4 : 2);
+    HYB_TRY(scratch.alloc_array(words, &bounds));
+    HYB_CUDA(cudaMemcpyAsync(bounds, predicate->value_id_bounds, sizeof(uint32_t) * words, cudaMemcpyHostToDevice,
                              context->stream));
     // value_id_bounds is borrowed pageable memory: the copy is staged before cudaMemcpyAsync returns.
-    device_predicate.value_id_bounds = static_cast<const uint32_t*>(*out_bounds_scratch);
-    if (out_uploaded_bytes) *out_uploaded_bytes = bytes;
+    device_predicate.value_id_bounds = bounds;
+    if (out_uploaded_bytes) *out_uploaded_bytes = sizeof(uint32_t) * words;
   }
-  void* tests = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(ChunkTest) * std::max<uint32_t>(chunk_count, 1), &tests));
+  ChunkTest* tests = nullptr;
+  HYB_TRY(scratch.alloc_array(chunk_count, &tests));
   if (chunk_count) {
     const DevSegment* column_segments = table->d_segments + size_t{predicate->column_id} * chunk_count;
-    scan_prepare_kernel<<<(chunk_count + 127) / 128, 128, 0, context->stream>>>(
-        column_segments, chunk_count, device_predicate, static_cast<ChunkTest*>(tests));
+    scan_prepare_kernel<<<(chunk_count + 127) / 128, 128, 0, context->stream>>>(column_segments, chunk_count,
+                                                                                device_predicate, tests);
     HYB_CUDA(cudaGetLastError());
   }
-  *out_tests = static_cast<ChunkTest*>(tests);
+  *out_bounds_scratch = scratch.release(bounds);
+  *out_tests = static_cast<ChunkTest*>(scratch.release(tests));
   return HYB_OK;
 }
 
@@ -1254,12 +1262,13 @@ static uint64_t column_bytes_per_launch(const Table* table, uint32_t column_id) 
 template <typename Rows>
 static int launch_two_pass(hyb_context* context, const ScanParams& params, const typename Rows::Extra& extra) {
   const uint32_t tile_count = params.tile_count;
+  DeviceScratch scratch(context);
   uint32_t* masks = nullptr;
   uint32_t* tile_counts = nullptr;
   unsigned long long* tile_bases = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint32_t) * size_t{tile_count} * kScanThreads, reinterpret_cast<void**>(&masks)));
-  HYB_TRY(device_alloc(context, sizeof(uint32_t) * size_t{tile_count}, reinterpret_cast<void**>(&tile_counts)));
-  HYB_TRY(device_alloc(context, sizeof(unsigned long long) * (size_t{tile_count} + 1), reinterpret_cast<void**>(&tile_bases)));
+  HYB_TRY(scratch.alloc_array(size_t{tile_count} * kScanThreads, &masks));
+  HYB_TRY(scratch.alloc_array(tile_count, &tile_counts));
+  HYB_TRY(scratch.alloc_array(size_t{tile_count} + 1, &tile_bases));
   int mask_blocks = 1, expand_blocks = 1;
   HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&mask_blocks, scan_mask_kernel<Rows>, kScanThreads, 0));
   HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&expand_blocks, scan_expand_kernel, kScanThreads, 0));
@@ -1268,9 +1277,6 @@ static int launch_two_pass(hyb_context* context, const ScanParams& params, const
   scan_bases_kernel<<<1, 1024, 0, context->stream>>>(tile_counts, tile_count, tile_bases);
   scan_expand_kernel<<<std::min<uint32_t>(tile_count, context->sm_count * std::max(expand_blocks, 1)), kScanThreads, 0,
                        context->stream>>>(params, masks, tile_bases);
-  device_free(context, masks);
-  device_free(context, tile_counts);
-  device_free(context, tile_bases);
   return HYB_OK;
 }
 
@@ -1281,21 +1287,19 @@ static int launch_filtered(hyb_context* context, const PosList* filter, const De
                            const ChunkTest* tests, const typename Rows::Extra& extra, bool null_row_matches,
                            PosList* result, uint64_t* out_input_rows) {
   const uint32_t chunk_count = result->chunk_count;
-  HYB_CUDA(cudaStreamSynchronize(context->stream));
   uint64_t input_count = 0;
-  HYB_CUDA(cudaMemcpy(&input_count, filter->d_chunk_end + filter->chunk_count, sizeof(uint64_t),
-                      cudaMemcpyDeviceToHost));
-  if (input_count == ~uint64_t{0}) input_count = 0;
+  HYB_TRY(pos_list_total(context, filter, &input_count));
   *out_input_rows = input_count;
   result->capacity = input_count;
   void* out = nullptr;
   HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * std::max<uint64_t>(input_count, 1), &out));
   result->d_row_ids = static_cast<hyb_row_id*>(out);
   const uint32_t tile_count = static_cast<uint32_t>((input_count + kFilteredTileRows - 1) / kFilteredTileRows);
-  void* status = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{tile_count} + 2), &status));
+  DeviceScratch scratch(context);
+  unsigned long long* status = nullptr;
+  HYB_TRY(scratch.alloc_array(size_t{tile_count} + 2, &status));
   HYB_CUDA(cudaMemsetAsync(status, 0, sizeof(uint64_t) * (size_t{tile_count} + 2), context->stream));
-  auto* total = static_cast<unsigned long long*>(status) + tile_count + 1;
+  unsigned long long* total = status + tile_count + 1;
   timing_kernel_begin(context);
   if (tile_count > 0) {
     FilteredScanParams params{};
@@ -1305,8 +1309,8 @@ static int launch_filtered(hyb_context* context, const PosList* filter, const De
     params.input_count = input_count;
     params.chunk_count = chunk_count;
     params.tile_count = tile_count;
-    params.tile_status = static_cast<unsigned long long*>(status);
-    params.ticket = reinterpret_cast<uint32_t*>(static_cast<unsigned long long*>(status) + tile_count);
+    params.tile_status = status;
+    params.ticket = reinterpret_cast<uint32_t*>(status + tile_count);
     params.out = result->d_row_ids;
     params.out_total = total;
     params.null_row_matches = null_row_matches;
@@ -1331,7 +1335,150 @@ static int launch_filtered(hyb_context* context, const PosList* filter, const De
     HYB_CUDA(cudaMemcpyAsync(result->d_chunk_end + 1, result->d_chunk_end, sizeof(uint64_t), cudaMemcpyDeviceToDevice, context->stream));
   }
   HYB_CUDA(cudaGetLastError());
-  device_free(context, status);
+  return HYB_OK;
+}
+
+// What an entry point prepared for run_scan.
+struct ScanPlan {
+  uint32_t row_column;        // the chunks' row counts come from this column's segments (ColumnRows: the scanned column)
+  const ChunkTest* tests;     // ColumnRows / InRows; nullptr otherwise
+  uint32_t prepare_launches;  // kernels counted before the scan's own
+  uint64_t prepared_bytes;    // uploaded lists / programs / translation words
+  uint64_t column_bytes;      // what one unfiltered pass reads (column_bytes_per_launch of every column read)
+  bool null_row_matches;      // filtered input: a NULL_ROW_ID satisfies the predicate
+};
+
+// The unfiltered scan over params.tile_count tiles; *launches grows by the kernels it starts. Only the one-column
+// predicate (ColumnRows, below) has the single-pass and bulk kernels: every other row evaluator takes the two-pass pipeline
+// whatever scan_two_pass / scan_bulk say.
+template <typename Rows>
+static int launch_unfiltered(hyb_context* context, const Table*, const ScanPlan&, const ScanParams& params,
+                             const typename Rows::Extra& extra, uint32_t* launches) {
+  if (context->options.trace && (!context->options.scan_two_pass || context->options.scan_bulk)) {
+    std::fprintf(stderr, "[hyb] table scan: two-pass pipeline (only one-column predicates have the single-pass and bulk "
+                         "kernels)\n");
+  }
+  timing_kernel_begin(context);
+  if (params.tile_count > 0) {
+    HYB_TRY(launch_two_pass<Rows>(context, params, extra));
+    *launches += 3;
+  }
+  timing_kernel_end(context);
+  return HYB_OK;
+}
+
+// One column against its ChunkTest: scan_two_pass selects the two-pass pipeline; otherwise scan_bulk selects the
+// TMA-staged kernel where every chunk streams a fixed-width vector of <= 4 bytes per row without a NULL vector, and
+// scan_kernel runs everywhere else.
+template <>
+int launch_unfiltered<ColumnRows>(hyb_context* context, const Table* table, const ScanPlan& plan, const ScanParams& column,
+                                  const ColumnRows::Extra& extra, uint32_t* launches) {
+  const uint32_t tile_count = column.tile_count;
+  if (tile_count == 0) {
+    timing_kernel_begin(context);
+    timing_kernel_end(context);
+    return HYB_OK;
+  }
+  DeviceScratch scratch(context);
+  unsigned long long* status = nullptr;  // look-back status per tile, then the ticket
+  HYB_TRY(scratch.alloc_array(size_t{tile_count} + 1, &status));
+  HYB_CUDA(cudaMemsetAsync(status, 0, sizeof(uint64_t) * (size_t{tile_count} + 1), context->stream));
+  ScanParams params = column;
+  params.tile_status = status;
+  params.ticket = reinterpret_cast<uint32_t*>(status + tile_count);
+  params.prefetch = 1;  // measured -8 % kernel time at SF 10
+  uint32_t stream_width = 0;
+  bool bulk = context->options.scan_bulk;
+  for (uint32_t chunk = 0; chunk < params.chunk_count && bulk; ++chunk) {
+    const DevSegment& segment = table->segments[size_t{chunk} * table->column_count + plan.row_column];
+    uint32_t width = 0;
+    if (segment.encoding == HYB_ENC_UNENCODED) {
+      width = static_cast<uint32_t>(data_type_size(segment.data_type));
+    } else {
+      width = segment.vector_type == HYB_VEC_FIXED_1B ? 1u : segment.vector_type == HYB_VEC_FIXED_2B ? 2u
+              : segment.vector_type == HYB_VEC_FIXED_4B ? 4u : 0u;
+    }
+    if (width == 0 || width > 4 || segment.nulls) bulk = false;
+    stream_width = std::max(stream_width, width);
+  }
+  timing_kernel_begin(context);
+  if (context->options.scan_two_pass) {
+    HYB_TRY(launch_two_pass<ColumnRows>(context, params, extra));
+    *launches += 3;
+  } else if (bulk) {
+    const uint32_t stage_bytes = kScanTileRows * stream_width;
+    const size_t dynamic_bytes = size_t{kBulkStages} * stage_bytes + sizeof(uint16_t) * kScanTileRows;
+    HYB_CUDA(cudaFuncSetAttribute(scan_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(dynamic_bytes)));
+    int blocks_per_sm = 0;
+    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, scan_bulk_kernel, kBulkThreads, dynamic_bytes));
+    const uint32_t grid = std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1));
+    scan_bulk_kernel<<<grid, kBulkThreads, dynamic_bytes, context->stream>>>(params, stage_bytes);
+    *launches += 1;
+  } else {
+    int blocks_per_sm = 0;
+    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, scan_kernel, kScanThreads, 0));
+    const uint32_t grid = std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1));
+    scan_kernel<<<grid, kScanThreads, 0, context->stream>>>(params);
+    *launches += 1;
+  }
+  timing_kernel_end(context);
+  return HYB_OK;
+}
+
+// Everything every scan entry point ends in: the result PosList, the unfiltered or the filtered launch, the operator
+// stats and the handle.
+template <typename Rows>
+static int run_scan(hyb_context* context, hyb_table_t table_handle, Table* table, const PosList* filter, const ScanPlan& plan,
+                    const typename Rows::Extra& extra, hyb_pos_list_t* out_pos_list) {
+  const uint32_t chunk_count = table->chunk_count();
+  const DevSegment* row_segments = table->d_segments + size_t{plan.row_column} * chunk_count;
+  auto result = std::make_unique<PosList>();
+  result->table = table_handle;
+  result->chunk_count = chunk_count;
+  result->stream = context->stream;
+  result->owner = context;
+  void* chunk_end = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
+  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
+  uint32_t launches = plan.prepare_launches;
+  uint64_t input_rows = 0, input_bytes = plan.prepared_bytes;
+
+  if (!filter) {
+    const uint2* tile_map = nullptr;
+    uint32_t tile_count = 0;
+    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
+    input_rows = table->row_count();
+    input_bytes += plan.column_bytes;
+    result->capacity = table->row_count();
+    void* out = nullptr;
+    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
+    result->d_row_ids = static_cast<hyb_row_id*>(out);
+    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
+    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
+    ScanParams params{};
+    params.segments = row_segments;
+    params.tests = plan.tests;
+    params.tile_map = tile_map;
+    params.chunk_count = chunk_count;
+    params.tile_count = tile_count;
+    params.out = result->d_row_ids;
+    params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
+    HYB_TRY(launch_unfiltered<Rows>(context, table, plan, params, extra, &launches));
+    HYB_CUDA(cudaGetLastError());
+  } else {
+    HYB_TRY(launch_filtered<Rows>(context, filter, row_segments, plan.tests, extra, plan.null_row_matches, result.get(),
+                                  &input_rows));
+    input_bytes += input_rows * sizeof(hyb_row_id);
+    launches += 2;  // filtered_scan_kernel, pos_list_chunk_ends_kernel
+  }
+  timing_end(context, launches, input_bytes, input_rows, 0);
+  // result->chunk_count: a filter in another order than the table's leaves one chunk
+  timing_output_count(context, result->d_chunk_end + result->chunk_count, sizeof(hyb_row_id));
+
+  const auto handle = context->next_handle++;
+  context->pos_lists.emplace(handle, std::move(result));
+  *out_pos_list = handle;
   return HYB_OK;
 }
 
@@ -1958,6 +2105,37 @@ std::string expression_tree_signature(const ExpressionTree& tree) {
   return signature;
 }
 
+// The table and the optional input_filter of a scan call (context->mutex held).
+static int find_scan_inputs(hyb_context* context, hyb_table_t table_handle, hyb_pos_list_t input_filter, Table** out_table,
+                            PosList** out_filter) {
+  *out_table = find_table(context, table_handle);
+  HYB_CHECK(*out_table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  *out_filter = nullptr;
+  if (input_filter) {
+    *out_filter = find_pos_list(context, input_filter);
+    HYB_CHECK(*out_filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
+    HYB_CHECK((*out_filter)->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
+  }
+  return HYB_OK;
+}
+
+// Launches the one-thread `kernel`: the predicate on a NULL_ROW_ID, every column NULL. With `read`, waits for its answer.
+template <typename Program>
+static int probe_null_row(hyb_context* context, DeviceScratch& scratch, void (*kernel)(Program, uint32_t*), Program program,
+                          bool read, bool* out_matches) {
+  uint32_t* d_matches = nullptr;
+  HYB_TRY(scratch.alloc_array(1, &d_matches));
+  kernel<<<1, 1, 0, context->stream>>>(program, d_matches);
+  HYB_CUDA(cudaGetLastError());
+  uint32_t matches = 0;
+  if (read) {
+    HYB_CUDA(cudaMemcpyAsync(&matches, d_matches, sizeof(uint32_t), cudaMemcpyDeviceToHost, context->stream));
+    HYB_CUDA(cudaStreamSynchronize(context->stream));
+  }
+  *out_matches = matches != 0;
+  return HYB_OK;
+}
+
 }  // namespace hyb
 
 using namespace hyb;
@@ -1970,119 +2148,25 @@ int hyb_table_scan(hyb_context* context, hyb_table_t table_handle, const hyb_sca
   *out_pos_list = 0;
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
-  auto* table = find_table(context, table_handle);
-  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  Table* table = nullptr;
   PosList* filter = nullptr;
-  if (input_filter) {
-    filter = find_pos_list(context, input_filter);
-    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
-    HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
-  }
+  HYB_TRY(find_scan_inputs(context, table_handle, input_filter, &table, &filter));
   HYB_TRY(sync_table_descriptors(context, table));
 
   timing_begin(context);
+  DeviceScratch scratch(context);
   ChunkTest* tests = nullptr;
   void* bounds_scratch = nullptr;
   HYB_TRY(prepare_chunk_tests(context, table, predicate, &tests, &bounds_scratch));
-
-  const uint32_t chunk_count = table->chunk_count();
-  auto result = std::make_unique<PosList>();
-  result->table = table_handle;
-  result->chunk_count = chunk_count;
-  result->stream = context->stream;
-  result->owner = context;
-  const DevSegment* column_segments = table->d_segments + size_t{predicate->column_id} * chunk_count;
-  uint32_t launches = 1;
-  uint64_t input_rows = 0, input_bytes = 0;
-
-  void* chunk_end = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
-  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
-
-  if (!filter) {
-    const uint2* tile_map = nullptr;
-    uint32_t tile_count = 0;
-    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
-    input_rows = table->row_count();
-    input_bytes = column_bytes_per_launch(table, predicate->column_id);
-    result->capacity = table->row_count();
-    void* out = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
-    result->d_row_ids = static_cast<hyb_row_id*>(out);
-    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
-    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
-    if (tile_count > 0) {
-      void* status = nullptr;
-      HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{tile_count} + 1), &status));
-      HYB_CUDA(cudaMemsetAsync(status, 0, sizeof(uint64_t) * (size_t{tile_count} + 1), context->stream));
-      ScanParams params{};
-      params.segments = column_segments;
-      params.tests = tests;
-      params.tile_map = tile_map;
-      params.chunk_count = chunk_count;
-      params.tile_count = tile_count;
-      params.tile_status = static_cast<unsigned long long*>(status);
-      params.ticket = reinterpret_cast<uint32_t*>(static_cast<unsigned long long*>(status) + tile_count);
-      params.out = result->d_row_ids;
-      params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
-      params.prefetch = 1;  // measured -8 % kernel time at SF 10
-      // Bulk (TMA-staged) path: every chunk streams a fixed-width vector of <= 4 bytes per row without a NULL vector.
-      uint32_t stream_width = 0;
-      bool bulk = context->options.scan_bulk;
-      for (uint32_t chunk = 0; chunk < chunk_count && bulk; ++chunk) {
-        const DevSegment& segment = table->segments[size_t{chunk} * table->column_count + predicate->column_id];
-        uint32_t width = 0;
-        if (segment.encoding == HYB_ENC_UNENCODED) {
-          width = static_cast<uint32_t>(data_type_size(segment.data_type));
-        } else {
-          width = segment.vector_type == HYB_VEC_FIXED_1B ? 1u : segment.vector_type == HYB_VEC_FIXED_2B ? 2u
-                  : segment.vector_type == HYB_VEC_FIXED_4B ? 4u : 0u;
-        }
-        if (width == 0 || width > 4 || segment.nulls) bulk = false;
-        stream_width = std::max(stream_width, width);
-      }
-      timing_kernel_begin(context);
-      if (context->options.scan_two_pass) {
-        HYB_TRY(launch_two_pass<ColumnRows>(context, params, ColumnRows::Extra{}));
-        launches = 4;
-      } else if (bulk) {
-        const uint32_t stage_bytes = kScanTileRows * stream_width;
-        const size_t dynamic_bytes = size_t{kBulkStages} * stage_bytes + sizeof(uint16_t) * kScanTileRows;
-        HYB_CUDA(cudaFuncSetAttribute(scan_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      static_cast<int>(dynamic_bytes)));
-        int blocks_per_sm = 0;
-        HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, scan_bulk_kernel, kBulkThreads, dynamic_bytes));
-        const uint32_t grid = std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1));
-        scan_bulk_kernel<<<grid, kBulkThreads, dynamic_bytes, context->stream>>>(params, stage_bytes);
-      } else {
-        int blocks_per_sm = 0;
-        HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, scan_kernel, kScanThreads, 0));
-        const uint32_t grid = std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1));
-        scan_kernel<<<grid, kScanThreads, 0, context->stream>>>(params);
-      }
-      timing_kernel_end(context);
-      HYB_CUDA(cudaGetLastError());
-      device_free(context, status);
-      launches = std::max<uint32_t>(launches, 2);
-    } else {
-      timing_kernel_begin(context);
-      timing_kernel_end(context);
-    }
-  } else {
-    HYB_TRY(launch_filtered<ColumnRows>(context, filter, column_segments, tests, ColumnRows::Extra{},
-                                        predicate->condition == HYB_PRED_IS_NULL, result.get(), &input_rows));
-    input_bytes = input_rows * sizeof(hyb_row_id);
-    launches = 3;
-  }
-  device_free(context, tests);
-  device_free(context, bounds_scratch);
-  timing_end(context, launches, input_bytes, input_rows, 0);
-  timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
-
-  const auto handle = context->next_handle++;
-  context->pos_lists.emplace(handle, std::move(result));
-  *out_pos_list = handle;
-  return HYB_OK;
+  scratch.adopt(tests);
+  scratch.adopt(bounds_scratch);
+  ScanPlan plan{};
+  plan.row_column = predicate->column_id;
+  plan.tests = tests;
+  plan.prepare_launches = 1;  // prepared_bytes stays 0: this call's stats have never counted the uploaded value_id_bounds
+  plan.column_bytes = column_bytes_per_launch(table, predicate->column_id);
+  plan.null_row_matches = predicate->condition == HYB_PRED_IS_NULL;
+  return run_scan<ColumnRows>(context, table_handle, table, filter, plan, ColumnRows::Extra{}, out_pos_list);
 }
 
 int hyb_table_scan_columns(hyb_context* context, hyb_table_t table_handle, const hyb_column_scan_predicate* predicate,
@@ -2091,14 +2175,9 @@ int hyb_table_scan_columns(hyb_context* context, hyb_table_t table_handle, const
   *out_pos_list = 0;
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
-  auto* table = find_table(context, table_handle);
-  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  Table* table = nullptr;
   PosList* filter = nullptr;
-  if (input_filter) {
-    filter = find_pos_list(context, input_filter);
-    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
-    HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
-  }
+  HYB_TRY(find_scan_inputs(context, table_handle, input_filter, &table, &filter));
   const int32_t condition = predicate->condition;
   HYB_CHECK(!is_like_condition(condition), HYB_ERR_UNSUPPORTED, "column-vs-column LIKE is not on the GPU path");
   HYB_CHECK(condition >= HYB_PRED_EQUALS && condition <= HYB_PRED_GREATER_THAN_EQUALS, HYB_ERR_INVALID,
@@ -2121,64 +2200,14 @@ int hyb_table_scan_columns(hyb_context* context, hyb_table_t table_handle, const
   uint64_t translation_words = 0;
   HYB_TRY(prepare_pair_tests(context, table, predicate, strings ? kCompareInt64 : pair_compare(left_type, right_type),
                              scratch, &tests, &translation_words));
-  const uint32_t chunk_count = table->chunk_count();
-  auto result = std::make_unique<PosList>();
-  result->table = table_handle;
-  result->chunk_count = chunk_count;
-  result->stream = context->stream;
-  result->owner = context;
-  const DevSegment* left_segments = table->d_segments + size_t{predicate->left_column_id} * chunk_count;
-  const PairRows::Extra extra{table->d_segments + size_t{predicate->right_column_id} * chunk_count, tests};
-  uint32_t launches = 1;
-  uint64_t input_rows = 0, input_bytes = sizeof(uint32_t) * translation_words;
-
-  void* chunk_end = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
-  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
-
-  if (!filter) {
-    // Column pairs only have the two-pass pipeline: scan_two_pass = 0 and scan_bulk select one-column kernels only.
-    if (context->options.trace && (!context->options.scan_two_pass || context->options.scan_bulk)) {
-      std::fprintf(stderr, "[hyb] hyb_table_scan_columns: two-pass pipeline (column pairs have no single-pass or bulk kernel)\n");
-    }
-    const uint2* tile_map = nullptr;
-    uint32_t tile_count = 0;
-    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
-    input_rows = table->row_count();
-    input_bytes += column_bytes_per_launch(table, predicate->left_column_id) +
-                   column_bytes_per_launch(table, predicate->right_column_id);
-    result->capacity = table->row_count();
-    void* out = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
-    result->d_row_ids = static_cast<hyb_row_id*>(out);
-    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
-    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
-    timing_kernel_begin(context);
-    if (tile_count > 0) {
-      ScanParams params{};
-      params.segments = left_segments;
-      params.tile_map = tile_map;
-      params.chunk_count = chunk_count;
-      params.tile_count = tile_count;
-      params.out = result->d_row_ids;
-      params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
-      HYB_TRY(launch_two_pass<PairRows>(context, params, extra));
-      launches = 4;
-    }
-    timing_kernel_end(context);
-    HYB_CUDA(cudaGetLastError());
-  } else {
-    HYB_TRY(launch_filtered<PairRows>(context, filter, left_segments, nullptr, extra, false, result.get(), &input_rows));
-    input_bytes += input_rows * sizeof(hyb_row_id);
-    launches = 3;
-  }
-  timing_end(context, launches, input_bytes, input_rows, 0);
-  timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
-
-  const auto handle = context->next_handle++;
-  context->pos_lists.emplace(handle, std::move(result));
-  *out_pos_list = handle;
-  return HYB_OK;
+  ScanPlan plan{};
+  plan.row_column = predicate->left_column_id;
+  plan.prepare_launches = 1;
+  plan.prepared_bytes = sizeof(uint32_t) * translation_words;
+  plan.column_bytes = column_bytes_per_launch(table, predicate->left_column_id) +
+                      column_bytes_per_launch(table, predicate->right_column_id);
+  const PairRows::Extra extra{table->d_segments + size_t{predicate->right_column_id} * table->chunk_count(), tests};
+  return run_scan<PairRows>(context, table_handle, table, filter, plan, extra, out_pos_list);
 }
 
 int hyb_table_scan_in(hyb_context* context, hyb_table_t table_handle, const hyb_in_predicate* predicate,
@@ -2187,14 +2216,9 @@ int hyb_table_scan_in(hyb_context* context, hyb_table_t table_handle, const hyb_
   *out_pos_list = 0;
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
-  auto* table = find_table(context, table_handle);
-  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  Table* table = nullptr;
   PosList* filter = nullptr;
-  if (input_filter) {
-    filter = find_pos_list(context, input_filter);
-    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
-    HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
-  }
+  HYB_TRY(find_scan_inputs(context, table_handle, input_filter, &table, &filter));
   InForm form;
   std::vector<hyb_value> bounds;
   HYB_TRY(check_in_predicate(table, predicate, &form, bounds));
@@ -2202,69 +2226,19 @@ int hyb_table_scan_in(hyb_context* context, hyb_table_t table_handle, const hyb_
 
   timing_begin(context);
   DeviceScratch scratch(context);
-  const uint32_t chunk_count = table->chunk_count();
-  const DevSegment* column_segments = table->d_segments + size_t{predicate->column_id} * chunk_count;
   ChunkTest* tests = nullptr;
   InList list{};
   uint64_t list_bytes = 0;
   HYB_TRY(prepare_in_tests(context, table, predicate, form, bounds, scratch, &tests, &list, &list_bytes));
-
-  auto result = std::make_unique<PosList>();
-  result->table = table_handle;
-  result->chunk_count = chunk_count;
-  result->stream = context->stream;
-  result->owner = context;
-  uint32_t launches = 1;
-  uint64_t input_rows = 0, input_bytes = list_bytes;
-  void* chunk_end = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
-  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
-
-  if (!filter) {
-    // IN lists only have the two-pass pipeline: scan_two_pass = 0 and scan_bulk select one-column kernels only.
-    if (context->options.trace && (!context->options.scan_two_pass || context->options.scan_bulk)) {
-      std::fprintf(stderr, "[hyb] hyb_table_scan_in: two-pass pipeline (IN lists have no single-pass or bulk kernel)\n");
-    }
-    const uint2* tile_map = nullptr;
-    uint32_t tile_count = 0;
-    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
-    input_rows = table->row_count();
-    input_bytes += column_bytes_per_launch(table, predicate->column_id);
-    result->capacity = table->row_count();
-    void* out = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
-    result->d_row_ids = static_cast<hyb_row_id*>(out);
-    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
-    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
-    timing_kernel_begin(context);
-    if (tile_count > 0) {
-      ScanParams params{};
-      params.segments = column_segments;
-      params.tests = tests;
-      params.tile_map = tile_map;
-      params.chunk_count = chunk_count;
-      params.tile_count = tile_count;
-      params.out = result->d_row_ids;
-      params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
-      HYB_TRY(launch_two_pass<InRows>(context, params, list));
-      launches = 4;
-    }
-    timing_kernel_end(context);
-    HYB_CUDA(cudaGetLastError());
-  } else {
-    // a NULL_ROW_ID reads as NULL: it matches only where NULL rows do, i.e. NOT IN over a list without a compatible element
-    HYB_TRY(launch_filtered<InRows>(context, filter, column_segments, tests, list, form == kInEveryRow, result.get(),
-                                    &input_rows));
-    input_bytes += input_rows * sizeof(hyb_row_id);
-    launches = 3;
-  }
-  timing_end(context, launches, input_bytes, input_rows, 0);
-  timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
-
-  const auto handle = context->next_handle++;
-  context->pos_lists.emplace(handle, std::move(result));
-  *out_pos_list = handle;
-  return HYB_OK;
+  ScanPlan plan{};
+  plan.row_column = predicate->column_id;
+  plan.tests = tests;
+  plan.prepare_launches = 1;
+  plan.prepared_bytes = list_bytes;
+  plan.column_bytes = column_bytes_per_launch(table, predicate->column_id);
+  // a NULL_ROW_ID reads as NULL: it matches only where NULL rows do, i.e. NOT IN over a list without a compatible element
+  plan.null_row_matches = form == kInEveryRow;
+  return run_scan<InRows>(context, table_handle, table, filter, plan, list, out_pos_list);
 }
 
 int hyb_table_scan_expression(hyb_context* context, hyb_table_t table_handle, const hyb_expression_scan_predicate* predicate,
@@ -2273,14 +2247,9 @@ int hyb_table_scan_expression(hyb_context* context, hyb_table_t table_handle, co
   *out_pos_list = 0;
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
-  auto* table = find_table(context, table_handle);
-  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  Table* table = nullptr;
   PosList* filter = nullptr;
-  if (input_filter) {
-    filter = find_pos_list(context, input_filter);
-    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
-    HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
-  }
+  HYB_TRY(find_scan_inputs(context, table_handle, input_filter, &table, &filter));
   auto program = std::make_unique<ExprProgram>();
   uint32_t column_ids[HYB_MAX_EXPRESSION_COLUMNS] = {};
   HYB_TRY(compile_expression(table, predicate, *program, column_ids));
@@ -2294,77 +2263,21 @@ int hyb_table_scan_expression(hyb_context* context, hyb_table_t table_handle, co
   }
   const size_t program_bytes = offsetof(ExprProgram, nodes) + sizeof(ExprNode) * program->node_count;
   void* d_program = nullptr;
-  uint32_t* d_null_row = nullptr;
   HYB_TRY(scratch.alloc(program_bytes, &d_program));
-  HYB_TRY(scratch.alloc_array(1, &d_null_row));
   // pageable source: the copy is staged before cudaMemcpyAsync returns
   HYB_CUDA(cudaMemcpyAsync(d_program, program.get(), program_bytes, cudaMemcpyHostToDevice, context->stream));
-  // every column NULL: the value of a NULL_ROW_ID, and of every row when the predicate reads no column
-  expression_null_row_kernel<<<1, 1, 0, context->stream>>>(static_cast<ExprProgram*>(d_program), d_null_row);
-  HYB_CUDA(cudaGetLastError());
-  const ExprProgram* extra = static_cast<const ExprProgram*>(d_program);
-
-  auto result = std::make_unique<PosList>();
-  result->table = table_handle;
-  result->chunk_count = chunk_count;
-  result->stream = context->stream;
-  result->owner = context;
-  uint32_t launches = 1;
-  uint64_t input_rows = 0, input_bytes = program_bytes;
-  void* chunk_end = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
-  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
-  // the segments of the first column read (any column when none is): ExprRows takes the chunks' row counts from them
-  const DevSegment* row_segments =
-      table->d_segments + size_t{program->column_count ? column_ids[0] : 0} * chunk_count;
-
-  if (!filter) {
-    // Expression predicates only have the two-pass pipeline: scan_two_pass = 0 and scan_bulk select one-column kernels only.
-    if (context->options.trace && (!context->options.scan_two_pass || context->options.scan_bulk)) {
-      std::fprintf(stderr, "[hyb] hyb_table_scan_expression: two-pass pipeline (expression predicates have no single-pass "
-                           "or bulk kernel)\n");
-    }
-    const uint2* tile_map = nullptr;
-    uint32_t tile_count = 0;
-    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
-    input_rows = table->row_count();
-    for (uint32_t c = 0; c < program->column_count; ++c) input_bytes += column_bytes_per_launch(table, column_ids[c]);
-    result->capacity = table->row_count();
-    void* out = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
-    result->d_row_ids = static_cast<hyb_row_id*>(out);
-    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
-    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
-    timing_kernel_begin(context);
-    if (tile_count > 0) {
-      ScanParams params{};
-      params.segments = row_segments;
-      params.tile_map = tile_map;
-      params.chunk_count = chunk_count;
-      params.tile_count = tile_count;
-      params.out = result->d_row_ids;
-      params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
-      HYB_TRY(launch_two_pass<ExprRows>(context, params, extra));
-      launches = 4;  // expression_null_row_kernel + the three two-pass kernels
-    }
-    timing_kernel_end(context);
-    HYB_CUDA(cudaGetLastError());
-  } else {
-    uint32_t null_row_matches = 0;
-    HYB_CUDA(cudaMemcpyAsync(&null_row_matches, d_null_row, sizeof(uint32_t), cudaMemcpyDeviceToHost, context->stream));
-    HYB_CUDA(cudaStreamSynchronize(context->stream));
-    HYB_TRY(launch_filtered<ExprRows>(context, filter, row_segments, nullptr, extra, null_row_matches != 0, result.get(),
-                                      &input_rows));
-    input_bytes += input_rows * sizeof(hyb_row_id);
-    launches = 3;  // expression_null_row_kernel, filtered_scan_kernel, pos_list_chunk_ends_kernel
-  }
-  timing_end(context, launches, input_bytes, input_rows, 0);
-  timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
-
-  const auto handle = context->next_handle++;
-  context->pos_lists.emplace(handle, std::move(result));
-  *out_pos_list = handle;
-  return HYB_OK;
+  ScanPlan plan{};
+  // every column NULL: the value of a NULL_ROW_ID, and of every row when the predicate reads no column (the kernel stores
+  // it in the program, so it runs unfiltered too)
+  HYB_TRY(probe_null_row(context, scratch, expression_null_row_kernel, static_cast<ExprProgram*>(d_program), filter != nullptr,
+                         &plan.null_row_matches));
+  // the first column read (any column when none is): ExprRows takes the chunks' row counts from its segments
+  plan.row_column = program->column_count ? column_ids[0] : 0;
+  plan.prepare_launches = 1;  // expression_null_row_kernel
+  plan.prepared_bytes = program_bytes;
+  for (uint32_t c = 0; c < program->column_count; ++c) plan.column_bytes += column_bytes_per_launch(table, column_ids[c]);
+  return run_scan<ExprRows>(context, table_handle, table, filter, plan, static_cast<const ExprProgram*>(d_program),
+                            out_pos_list);
 }
 
 int hyb_table_scan_expression_tests(hyb_context* context, hyb_table_t table_handle,
@@ -2379,14 +2292,9 @@ int hyb_table_scan_expression_tests(hyb_context* context, hyb_table_t table_hand
 
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
-  auto* table = find_table(context, table_handle);
-  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  Table* table = nullptr;
   PosList* filter = nullptr;
-  if (input_filter) {
-    filter = find_pos_list(context, input_filter);
-    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown input_filter handle");
-    HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
-  }
+  HYB_TRY(find_scan_inputs(context, table_handle, input_filter, &table, &filter));
   // host checks of every leaf before anything runs
   auto tree = std::make_unique<ExpressionTree>();
   HYB_TRY(compile_expression_tree(table, predicate, leaf_tests, tree.get()));
@@ -2394,101 +2302,32 @@ int hyb_table_scan_expression_tests(hyb_context* context, hyb_table_t table_hand
 
   timing_begin(context);
   DeviceScratch scratch(context);
-  const uint32_t chunk_count = table->chunk_count();
   HYB_TRY(upload_expression_tree(context, table, *tree, scratch));
-  const TestProgram* host = &tree->host;
-  const ExprProgram* program = &tree->program;
-  const uint32_t* test_columns = tree->test_columns;
-  const uint32_t* column_ids = tree->column_ids;
   const bool operands = tree->operands();
-  uint32_t launches = tree->launches;
-  const TestProgram* d_tests = tree->device;
-  const TestProgram* extra = d_tests;
-
+  ScanPlan plan{};
+  plan.prepare_launches = tree->launches;
+  if (filter) {
+    HYB_TRY(probe_null_row(context, scratch,
+                           operands ? expression_tests_null_row_kernel<true> : expression_tests_null_row_kernel<false>,
+                           tree->device, true, &plan.null_row_matches));
+    ++plan.prepare_launches;
+  }
+  // the first test leaf's column: TestRows takes the chunks' row counts from its segments
+  plan.row_column = tree->test_columns[0];
+  plan.prepared_bytes = tree->uploaded_bytes;
   // every distinct column once, whether an operand or a test leaf reads it
-  uint64_t input_rows = 0, input_bytes = tree->uploaded_bytes;
-  uint64_t column_bytes = 0;
-  for (uint32_t c = 0; c < host->column_count; ++c) column_bytes += column_bytes_per_launch(table, test_columns[c]);
-  for (uint32_t c = 0; c < program->column_count; ++c) {
-    if (std::find(test_columns, test_columns + host->column_count, column_ids[c]) == test_columns + host->column_count) {
-      column_bytes += column_bytes_per_launch(table, column_ids[c]);
+  const uint32_t* test_columns = tree->test_columns;
+  const uint32_t test_column_count = tree->host.column_count;
+  for (uint32_t c = 0; c < test_column_count; ++c) plan.column_bytes += column_bytes_per_launch(table, test_columns[c]);
+  for (uint32_t c = 0; c < tree->program.column_count; ++c) {
+    const uint32_t column_id = tree->column_ids[c];
+    if (std::find(test_columns, test_columns + test_column_count, column_id) == test_columns + test_column_count) {
+      plan.column_bytes += column_bytes_per_launch(table, column_id);
     }
   }
-
-  auto result = std::make_unique<PosList>();
-  result->table = table_handle;
-  result->chunk_count = chunk_count;
-  result->stream = context->stream;
-  result->owner = context;
-  void* chunk_end = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{chunk_count} + 1), &chunk_end));
-  result->d_chunk_end = static_cast<uint64_t*>(chunk_end);
-  // the segments of the first test leaf's column: TestRows takes the chunks' row counts from them
-  const DevSegment* row_segments = host->columns[0];
-
-  if (!filter) {
-    if (context->options.trace && (!context->options.scan_two_pass || context->options.scan_bulk)) {
-      std::fprintf(stderr, "[hyb] hyb_table_scan_expression_tests: two-pass pipeline (expression predicates have no "
-                           "single-pass or bulk kernel)\n");
-    }
-    const uint2* tile_map = nullptr;
-    uint32_t tile_count = 0;
-    HYB_TRY(get_tile_map(context, table, kScanTileRows, &tile_map, &tile_count));
-    input_rows = table->row_count();
-    input_bytes += column_bytes;
-    result->capacity = table->row_count();
-    void* out = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * result->capacity, &out));
-    result->d_row_ids = static_cast<hyb_row_id*>(out);
-    // chunk_end is pre-filled with "unset" so chunks without rows can be patched on the host.
-    HYB_CUDA(cudaMemsetAsync(chunk_end, 0xFF, sizeof(uint64_t) * (size_t{chunk_count} + 1), context->stream));
-    timing_kernel_begin(context);
-    if (tile_count > 0) {
-      ScanParams params{};
-      params.segments = row_segments;
-      params.tile_map = tile_map;
-      params.chunk_count = chunk_count;
-      params.tile_count = tile_count;
-      params.out = result->d_row_ids;
-      params.chunk_end = reinterpret_cast<unsigned long long*>(result->d_chunk_end);
-      if (operands) {
-        HYB_TRY(launch_two_pass<TestRows<true>>(context, params, extra));
-      } else {
-        HYB_TRY(launch_two_pass<TestRows<false>>(context, params, extra));
-      }
-      launches += 3;
-    }
-    timing_kernel_end(context);
-    HYB_CUDA(cudaGetLastError());
-  } else {
-    uint32_t* d_null_row = nullptr;
-    HYB_TRY(scratch.alloc_array(1, &d_null_row));
-    if (operands) {
-      expression_tests_null_row_kernel<true><<<1, 1, 0, context->stream>>>(d_tests, d_null_row);
-    } else {
-      expression_tests_null_row_kernel<false><<<1, 1, 0, context->stream>>>(d_tests, d_null_row);
-    }
-    HYB_CUDA(cudaGetLastError());
-    uint32_t null_row_matches = 0;
-    HYB_CUDA(cudaMemcpyAsync(&null_row_matches, d_null_row, sizeof(uint32_t), cudaMemcpyDeviceToHost, context->stream));
-    HYB_CUDA(cudaStreamSynchronize(context->stream));
-    if (operands) {
-      HYB_TRY(launch_filtered<TestRows<true>>(context, filter, row_segments, nullptr, extra, null_row_matches != 0,
-                                              result.get(), &input_rows));
-    } else {
-      HYB_TRY(launch_filtered<TestRows<false>>(context, filter, row_segments, nullptr, extra, null_row_matches != 0,
-                                               result.get(), &input_rows));
-    }
-    input_bytes += input_rows * sizeof(hyb_row_id);
-    launches += 3;  // the null-row kernel, filtered_scan_kernel, pos_list_chunk_ends_kernel
-  }
-  timing_end(context, launches, input_bytes, input_rows, 0);
-  timing_output_count(context, result->d_chunk_end + chunk_count, sizeof(hyb_row_id));
+  HYB_TRY(operands ? run_scan<TestRows<true>>(context, table_handle, table, filter, plan, tree->device, out_pos_list)
+                   : run_scan<TestRows<false>>(context, table_handle, table, filter, plan, tree->device, out_pos_list));
   context->timing.stats.path = operands ? 2 : 1;
-
-  const auto handle = context->next_handle++;
-  context->pos_lists.emplace(handle, std::move(result));
-  *out_pos_list = handle;
   return HYB_OK;
 }
 

@@ -559,11 +559,7 @@ int hyb_sort(hyb_context* context, hyb_table_t table_handle, hyb_pos_list_t inpu
     HYB_CHECK(filter->table == table_handle, HYB_ERR_INVALID, "input_filter belongs to a different table");
   }
   uint64_t rows = table->row_count();
-  if (filter) {
-    HYB_CUDA(cudaMemcpyAsync(&rows, filter->d_chunk_end + filter->chunk_count, sizeof(uint64_t), cudaMemcpyDeviceToHost,
-                             context->stream));
-    HYB_CUDA(cudaStreamSynchronize(context->stream));
-  }
+  if (filter) HYB_TRY(pos_list_total(context, filter, &rows));
   HYB_CHECK(rows < 0xFFFFFFFFull, HYB_ERR_UNSUPPORTED, "sorting 2^32 or more rows runs on the CPU operator");
   HYB_TRY(sync_table_descriptors(context, table));
   const uint32_t count = static_cast<uint32_t>(rows);
