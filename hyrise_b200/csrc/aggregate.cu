@@ -1738,10 +1738,6 @@ static double double_from_ordered(uint64_t ordered) {
 
 using namespace hyb;
 
-extern "C" {
-
-}  // extern "C"
-
 static int exchange_partial_groups(hyb_context* context, const AggregateExchange& exchange, const Table* table,
                                    const hyb_aggregate_query* query, const std::vector<int32_t>& input_types,
                                    std::vector<HostGroup>* groups, bool* out_needs_partitioning);
@@ -1881,75 +1877,34 @@ static std::string aggregate_signature(const hyb_aggregate_query* query) {
   return signature;
 }
 
-// hyb_aggregate_hash with context->mutex held. `exchange` != nullptr: the groups of this rank are partial; they are
-// exchanged with the peer group's ranks and merged before the result is ordered and materialised. `tree` != nullptr: a
-// compiled expression tree (hyb_aggregate_hash_expression) every aggregated row must also satisfy.
-static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query* query, hyb_aggregate_result_t* out_result,
-                                 const AggregateExchange* exchange, ExpressionTree* tree = nullptr) {
-  auto* table = find_table(context, query->table);
-  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
-  PosList* filter = nullptr;
-  if (query->filter) {
-    filter = find_pos_list(context, query->filter);
-    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown filter handle");
-    HYB_CHECK(filter->table == query->table, HYB_ERR_INVALID, "filter belongs to a different table");
-    HYB_CHECK(!filter->may_hold_null_rows, HYB_ERR_UNSUPPORTED,
-              "aggregating a PosList with NULL_ROW_IDs (an outer join's output) runs on the CPU operator");
-  }
-  HYB_TRY(sync_table_descriptors(context, table));
-  cudaStream_t stream = context->stream;
-  const uint32_t chunk_count = table->chunk_count();
-  const uint32_t aggregate_count = query->aggregate_count;
+// Whether an aggregate's expression reads a string column of `table` (a column out of range is rejected when it is typed).
+static bool has_string_argument(const Table* table, const hyb_aggregate_def& def) {
+  return std::any_of(def.nodes, def.nodes + def.node_count, [&](const auto& node) {
+    return node.op == HYB_EXPR_COLUMN && node.column_id < table->column_count &&
+           table->column_types[node.column_id] == HYB_TYPE_STRING;
+  });
+}
 
-  // ---- ANY: a group-by column the shim writes from the representative RowIDs (write_groupby_output, :421-537) -------
-  // It adds no accumulator: the other aggregates run exactly as without it (an all-ANY query is the group-by-only call,
-  // the reference's DISTINCT path), and its column of the result only names its type.
-  std::vector<hyb_aggregate_def> kept;
-  std::vector<int32_t> any_types(aggregate_count, -1);
-  for (uint32_t a = 0; a < aggregate_count; ++a) {
-    const auto& def = query->aggregates[a];
-    if (def.function != HYB_AGG_ANY) {
-      kept.push_back(def);
-      continue;
-    }
-    HYB_CHECK(def.node_count == 1 && def.nodes[0].op == HYB_EXPR_COLUMN && def.nodes[0].column_id < table->column_count,
-              HYB_ERR_INVALID, "ANY takes a single column of the input table");
-    any_types[a] = table->column_types[def.nodes[0].column_id];
-  }
-  if (kept.size() < aggregate_count) {
-    hyb_aggregate_query reduced = *query;
-    reduced.aggregate_count = static_cast<uint32_t>(kept.size());
-    reduced.aggregates = kept.data();
-    HYB_TRY(aggregate_hash_locked(context, &reduced, out_result, exchange, tree));
-    auto& result = *context->aggregate_results.at(*out_result);
-    std::vector<AggregateColumn> columns(aggregate_count);
-    for (uint32_t a = 0, next = 0; a < aggregate_count; ++a) {
-      if (any_types[a] >= 0) {
-        columns[a].value_type = any_types[a];
-        columns[a].is_any = true;
-      } else {
-        columns[a] = std::move(result.columns[next++]);
-      }
-    }
-    result.columns = std::move(columns);
-    return HYB_OK;
-  }
-
-  // ---- validate + type the aggregates -----------------------------------------------------------------------------
-  std::vector<int32_t> input_types(aggregate_count, HYB_TYPE_INT64), result_types(aggregate_count, HYB_TYPE_INT64);
+struct AggregateTypes {
+  std::vector<int32_t> input_types, result_types;
   // MIN / MAX / COUNT of a bare string column: the column's INT32 view (order ranks, or zeros for COUNT)
-  std::vector<Table::StringColumnView*> string_views(aggregate_count, nullptr);
+  std::vector<Table::StringColumnView*> string_views;
+};
+
+// Validates the aggregates (ANY already stripped) and the group-by columns, and types every aggregate.
+static int type_aggregates(hyb_context* context, Table* table, const hyb_aggregate_query* query, AggregateTypes* out) {
+  const uint32_t aggregate_count = query->aggregate_count;
+  const uint32_t chunk_count = table->chunk_count();
+  out->input_types.assign(aggregate_count, HYB_TYPE_INT64);
+  out->result_types.assign(aggregate_count, HYB_TYPE_INT64);
+  out->string_views.assign(aggregate_count, nullptr);
   for (uint32_t a = 0; a < aggregate_count; ++a) {
     const auto& def = query->aggregates[a];
     HYB_CHECK(def.function >= HYB_AGG_MIN && def.function <= HYB_AGG_STDDEV_SAMP, HYB_ERR_UNSUPPORTED,
               "aggregate function " + std::to_string(def.function) + " runs on the CPU operator");
     if (def.function == HYB_AGG_COUNT_STAR) continue;
     HYB_CHECK(def.node_count >= 1 && def.node_count <= HYB_MAX_EXPR_NODES, HYB_ERR_INVALID, "bad expression length");
-    bool string_argument = false;
-    for (uint32_t n = 0; n < def.node_count; ++n) {
-      string_argument |= def.nodes[n].op == HYB_EXPR_COLUMN && def.nodes[n].column_id < table->column_count &&
-                         table->column_types[def.nodes[n].column_id] == HYB_TYPE_STRING;
-    }
+    const bool string_argument = has_string_argument(table, def);
     if (string_argument && def.function == HYB_AGG_STDDEV_SAMP) {
       HYB_CHECK(false, HYB_ERR_INVALID, "STDDEV_SAMP is not defined for strings");
     }
@@ -1963,20 +1918,21 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
         HYB_CHECK(segment.encoding == HYB_ENC_DICTIONARY && segment.dict_codes, HYB_ERR_UNSUPPORTED,
                   "COUNT(DISTINCT) over a string column needs dictionary_codes in its segments");
       }
-      input_types[a] = HYB_TYPE_STRING;
-      result_types[a] = HYB_TYPE_INT64;
+      out->input_types[a] = HYB_TYPE_STRING;
+      out->result_types[a] = HYB_TYPE_INT64;
       continue;
     }
     const bool bare_column = def.node_count == 1 && def.nodes[0].op == HYB_EXPR_COLUMN;
     if (string_argument && bare_column &&
         (def.function == HYB_AGG_MIN || def.function == HYB_AGG_MAX || def.function == HYB_AGG_COUNT)) {
-      HYB_TRY(string_column_view(context, table, def.nodes[0].column_id, def.function != HYB_AGG_COUNT, &string_views[a]));
-      input_types[a] = HYB_TYPE_STRING;
-      result_types[a] = def.function == HYB_AGG_COUNT ? HYB_TYPE_INT64 : HYB_TYPE_STRING;
+      HYB_TRY(string_column_view(context, table, def.nodes[0].column_id, def.function != HYB_AGG_COUNT,
+                                 &out->string_views[a]));
+      out->input_types[a] = HYB_TYPE_STRING;
+      out->result_types[a] = def.function == HYB_AGG_COUNT ? HYB_TYPE_INT64 : HYB_TYPE_STRING;
       continue;
     }
-    HYB_TRY(expression_type(table, def, &input_types[a]));
-    result_types[a] = aggregate_result_type(def.function, input_types[a]);
+    HYB_TRY(expression_type(table, def, &out->input_types[a]));
+    out->result_types[a] = aggregate_result_type(def.function, out->input_types[a]);
   }
   for (uint32_t g = 0; g < query->groupby_count; ++g) {
     const uint32_t column = query->groupby_column_ids[g];
@@ -1988,50 +1944,54 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
       }
     }
   }
+  return HYB_OK;
+}
 
-  timing_begin(context);
-  uint32_t launches = 0;
+struct FusedPredicates {
+  std::vector<ChunkTest*> tests;      // per fused predicate
+  const TestProgram* tree = nullptr;  // the expression tree's programs (hyb_aggregate_hash_expression), or none
+  uint32_t launches = 0;              // the kernels that built the tests
+};
 
-  // ---- fused predicates -------------------------------------------------------------------------------------------
-  std::vector<ChunkTest*> tests(query->predicate_count, nullptr);
-  std::vector<void*> bounds(query->predicate_count, nullptr);
-  const auto release_tests = [&]() {
-    for (auto* t : tests) device_free(context, t);
-    for (auto* b : bounds) device_free(context, b);
-  };
+// The fused predicates' per-chunk tests and the expression tree's tests and programs, all owned by `scratch`.
+static int prepare_fused_predicates(hyb_context* context, Table* table, const hyb_aggregate_query* query,
+                                    ExpressionTree* tree, DeviceScratch& scratch, FusedPredicates* out) {
+  out->tests.assign(query->predicate_count, nullptr);
   for (uint32_t p = 0; p < query->predicate_count; ++p) {
-    const int status = prepare_chunk_tests(context, table, &query->predicates[p], &tests[p], &bounds[p]);
-    if (status != HYB_OK) {
-      release_tests();
-      return status;
-    }
-    ++launches;
+    void* bounds = nullptr;
+    HYB_TRY(prepare_chunk_tests(context, table, &query->predicates[p], &out->tests[p], &bounds));
+    scratch.adopt(out->tests[p]);
+    scratch.adopt(bounds);
+    ++out->launches;
   }
-  DeviceScratch tree_scratch(context);
   if (tree) {
-    if (const int status = upload_expression_tree(context, table, *tree, tree_scratch); status != HYB_OK) {
-      release_tests();
-      return status;
+    HYB_TRY(upload_expression_tree(context, table, *tree, scratch));
+    out->tree = tree->device;
+    out->launches += tree->launches;
+  }
+  return HYB_OK;
+}
+
+// The rank words string MIN / MAX read as their dictionaries, each view once (`ordered_only`: views with ranks only).
+static uint64_t rank_word_bytes(const AggregateTypes& types, bool ordered_only) {
+  std::vector<const Table::StringColumnView*> ranked;
+  uint64_t bytes = 0;
+  for (size_t a = 0; a < types.string_views.size(); ++a) {
+    const Table::StringColumnView* view = types.string_views[a];
+    if (view && (!ordered_only || view->ordered) && types.result_types[a] == HYB_TYPE_STRING &&
+        std::find(ranked.begin(), ranked.end(), view) == ranked.end()) {
+      ranked.push_back(view);
+      bytes += sizeof(uint32_t) * view->word_count;
     }
-    launches += tree->launches;
   }
-  const TestProgram* tree_program = tree ? tree->device : nullptr;
+  return bytes;
+}
 
-  uint64_t position_count = table->row_count();
-  if (filter) HYB_TRY(pos_list_total(context, filter, &position_count));
-
-  std::vector<HostGroup> groups;
-  bool done = false;
-  uint32_t path = HYB_AGG_PATH_NONE;  // hyb_operator_stats::path: the kernel whose groups are returned
-  int forced_immediate = -1;
-  uint64_t algorithmic_bytes = 0;
-  std::shared_ptr<AggregatePlanMemo> memo;
-  {
-    auto& slot = table->plan_memo[tree ? aggregate_signature(query) + "tree" + expression_tree_signature(*tree)
-                                       : aggregate_signature(query)];
-    if (!slot) slot = std::make_shared<AggregatePlanMemo>();
-    memo = std::static_pointer_cast<AggregatePlanMemo>(slot);
-  }
+// hyb_operator_stats::algorithmic_bytes: every referenced column once (kept in the memo), or one RowID per position of
+// a filtered input; plus the expression tree's uploads and, on filtered inputs, the rank words.
+static uint64_t aggregate_algorithmic_bytes(const Table* table, const hyb_aggregate_query* query, const ExpressionTree* tree,
+                                            const AggregateTypes& types, const PosList* filter, uint64_t position_count,
+                                            AggregatePlanMemo* memo) {
   if (memo->algorithmic_bytes == 0) {
     // bytes of every referenced column, each counted once
     std::vector<uint32_t> referenced;
@@ -2041,7 +2001,7 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
       referenced.insert(referenced.end(), tree->test_columns, tree->test_columns + tree->host.column_count);
       referenced.insert(referenced.end(), tree->column_ids, tree->column_ids + tree->program.column_count);
     }
-    for (uint32_t a = 0; a < aggregate_count; ++a) {
+    for (uint32_t a = 0; a < query->aggregate_count; ++a) {
       for (uint32_t n = 0; n < query->aggregates[a].node_count; ++n) {
         if (query->aggregates[a].nodes[n].op == HYB_EXPR_COLUMN) referenced.push_back(query->aggregates[a].nodes[n].column_id);
       }
@@ -2049,7 +2009,7 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
     std::sort(referenced.begin(), referenced.end());
     referenced.erase(std::unique(referenced.begin(), referenced.end()), referenced.end());
     for (const uint32_t column : referenced) {
-      for (uint32_t chunk = 0; chunk < chunk_count; ++chunk) {
+      for (uint32_t chunk = 0; chunk < table->chunk_count(); ++chunk) {
         const auto& segment = table->segments[size_t{chunk} * table->column_count + column];
         if (segment.encoding == HYB_ENC_UNENCODED) {
           memo->algorithmic_bytes += data_type_size(segment.data_type) * segment.row_count;
@@ -2065,126 +2025,220 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
         if (segment.nulls) memo->algorithmic_bytes += segment.row_count;
       }
     }
-    // string MIN / MAX read the column's rank words as its dictionaries
-    std::vector<const Table::StringColumnView*> ranked;
-    for (uint32_t a = 0; a < aggregate_count; ++a) {
-      if (string_views[a] && string_views[a]->ordered && result_types[a] == HYB_TYPE_STRING &&
-          std::find(ranked.begin(), ranked.end(), string_views[a]) == ranked.end()) {
-        ranked.push_back(string_views[a]);
-        memo->algorithmic_bytes += sizeof(uint32_t) * string_views[a]->word_count;
-      }
-    }
+    memo->algorithmic_bytes += rank_word_bytes(types, true);  // string MIN / MAX read the column's rank words
   }
-  algorithmic_bytes = filter ? position_count * sizeof(hyb_row_id) : memo->algorithmic_bytes;
-  if (tree) algorithmic_bytes += tree->uploaded_bytes;  // the leaves' tests, bitmaps and intervals, and the programs
-  if (filter) {  // string MIN / MAX read their rank words as dictionaries on filtered inputs too
-    std::vector<const Table::StringColumnView*> ranked;
-    for (uint32_t a = 0; a < aggregate_count; ++a) {
-      if (string_views[a] && result_types[a] == HYB_TYPE_STRING &&
-          std::find(ranked.begin(), ranked.end(), string_views[a]) == ranked.end()) {
-        ranked.push_back(string_views[a]);
-        algorithmic_bytes += sizeof(uint32_t) * string_views[a]->word_count;
-      }
-    }
+  uint64_t bytes = filter ? position_count * sizeof(hyb_row_id) : memo->algorithmic_bytes;
+  if (tree) bytes += tree->uploaded_bytes;       // the leaves' tests, bitmaps and intervals, and the programs
+  if (filter) bytes += rank_word_bytes(types, false);  // string MIN / MAX read their rank words on filtered inputs too
+  return bytes;
+}
+
+// What both kernels' plans read besides their own fields: the fused predicates' segments and tests, the group-by segments.
+template <typename Plan>
+static void plan_inputs(const Table* table, const hyb_aggregate_query* query, const FusedPredicates& fused, Plan* plan) {
+  const uint32_t chunk_count = table->chunk_count();
+  plan->chunk_row_start = reinterpret_cast<const unsigned long long*>(table->d_chunk_row_start);
+  plan->predicate_count = query->predicate_count;
+  for (uint32_t p = 0; p < query->predicate_count; ++p) {
+    plan->predicate_segments[p] = table->d_segments + size_t{query->predicates[p].column_id} * chunk_count;
+    plan->predicate_tests[p] = fused.tests[p];
   }
+  plan->groupby_count = query->groupby_count;
+  for (uint32_t g = 0; g < query->groupby_count; ++g) {
+    plan->group_segments[g] = table->d_segments + size_t{query->groupby_column_ids[g]} * chunk_count;
+  }
+}
+
+// This rank's groups, the kernel they came from (hyb_operator_stats::path), the launches so far and the timed span.
+struct AggregateOutcome {
+  bool done = false;
+  std::vector<HostGroup> groups;
+  uint32_t path = HYB_AGG_PATH_NONE;
+  uint32_t launches = 0;
   bool kernel_timed = false;
+};
 
-  // ---- fast path --------------------------------------------------------------------------------------------------
-  const FastPlanHost fast = plan_fast_path(table, query);
-  if (fast.possible && chunk_count > 0) {
-    const int column_template = fast.columns.size() <= 1 ? 1 : fast.columns.size() <= 2 ? 2 : 4;
-    // Attempts in order: the TMA-staged streaming kernel when the layout allows it (<= 4 groups), then the register-tile
-    // kernel with 4 and 8 group slots; a kernel that meets more groups than it has slots raises `overflow`.
-    struct Attempt {
-      bool stream;
-      int groups;
-    };
-    std::vector<Attempt> attempts;
-    StreamLayout stream_layout;
-    if (context->options.aggregate_stream) {
-      if (!memo->has_stream_layout || memo->stream_stages != context->options.aggregate_stages) {
-        memo->stream_layout = stream_layout_for(table, query, fast, context->options.aggregate_stages, tree != nullptr);
-        memo->stream_stages = context->options.aggregate_stages;
-        memo->has_stream_layout = true;
+// Offsets (64-bit words) in the fast path's partials block of `entries` (CTA x group slot) entries and C value columns.
+// The copy back to the host covers all `words`; the device FastPlan follows them.
+struct FastPartials {
+  size_t hash, keys, rows, min_position, max_position, raw, product, raw_nulls, product_nulls, null_mask, overflow, words;
+  FastPartials(size_t entries, size_t C)
+      : hash(0), keys(hash + entries), rows(keys + entries * kMaxKeyWords), min_position(rows + entries),
+        max_position(min_position + entries), raw(max_position + entries), product(raw + entries * C),
+        raw_nulls(product + entries * C), product_nulls(raw_nulls + entries * C), null_mask(product_nulls + entries * C),
+        overflow(null_mask + (entries + 1) / 2), words(overflow + 1) {}
+};
+
+// Merges the per-CTA partials in CTA order (deterministic). false: two groups share a 64-bit hash.
+static bool merge_fast_partials(const hyb_aggregate_query* query, const FastPlanHost& fast, const std::vector<uint64_t>& host,
+                                const FastPartials& layout, size_t entries, int C, std::vector<HostGroup>* groups) {
+  struct Merged {
+    uint64_t hash;
+    std::vector<uint64_t> key;
+    uint32_t null_mask;
+    uint64_t rows = 0, min_position = ~uint64_t{0}, max_position = 0;
+    std::vector<double> raw_f, product_f;
+    std::vector<int64_t> raw_i;
+    std::vector<uint64_t> raw_nulls, product_nulls;
+  };
+  const auto* null_masks = reinterpret_cast<const uint32_t*>(&host[layout.null_mask]);
+  std::vector<Merged> merged;
+  bool consistent = true;
+  for (size_t entry = 0; entry < entries; ++entry) {
+    const uint64_t hash = host[layout.hash + entry];
+    if (hash == 0 || host[layout.rows + entry] == 0) continue;
+    const uint64_t* key_words = &host[layout.keys + entry * kMaxKeyWords];
+    std::vector<uint64_t> key(key_words, key_words + std::max<uint32_t>(query->groupby_count, 1));
+    Merged* target = nullptr;
+    for (auto& m : merged) {
+      if (m.hash == hash) {
+        if (m.key != key || m.null_mask != null_masks[entry]) consistent = false;  // 64-bit hash collision
+        target = &m;
       }
-      stream_layout = memo->stream_layout;
     }
-    if (stream_layout.possible) attempts.push_back({true, query->groupby_count == 0 ? 1 : 4});
-    if (query->groupby_count == 0) {
-      attempts.push_back({false, 1});
-    } else {
-      attempts.push_back({false, 4});
-      attempts.push_back({false, 8});
+    if (!target) {
+      merged.emplace_back();
+      target = &merged.back();
+      target->hash = hash;
+      target->key = key;
+      target->null_mask = null_masks[entry];
+      target->raw_f.assign(C, 0.0);
+      target->product_f.assign(C, 0.0);
+      target->raw_i.assign(C, 0);
+      target->raw_nulls.assign(C, 0);
+      target->product_nulls.assign(C, 0);
     }
-    for (const Attempt attempt : attempts) {
-      const uint2* tile_map = nullptr;
-      uint32_t tile_count = 0;
-      HYB_TRY(get_tile_map(context, table, attempt.stream ? kStreamTileRows : kAggTileRows, &tile_map, &tile_count));
-      const int G = attempt.groups;
-      const int C = column_template;
-      const FastKernel kernel = fast_kernel(fast.work_type, G, C, tree != nullptr);
-      uint32_t grid = 1;
-      if (attempt.stream) {
-        // one persistent CTA per SM; its tiles are kStreamRounds contiguous runs, the runs strided over the CTAs
-        grid = std::max<uint32_t>(1, std::min<uint32_t>(tile_count, context->sm_count));
+    target->rows += host[layout.rows + entry];
+    target->min_position = std::min(target->min_position, host[layout.min_position + entry]);
+    target->max_position = std::max(target->max_position, host[layout.max_position + entry]);
+    for (int c = 0; c < C; ++c) {
+      const size_t at = entry * C + c;
+      if (fast.work_type == 2) {
+        target->raw_i[c] += static_cast<int64_t>(host[layout.raw + at]);
       } else {
-        int blocks_per_sm = 1;
-        HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kernel, kFastThreads, 0));
-        // one wave of resident CTAs: the static tile striding must not queue CTAs behind each other
-        grid = std::max<uint32_t>(1, std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1)));
+        double raw, product;
+        std::memcpy(&raw, &host[layout.raw + at], sizeof(double));
+        std::memcpy(&product, &host[layout.product + at], sizeof(double));
+        target->raw_f[c] += raw;
+        target->product_f[c] += product;
       }
-      FastPlan host_plan{};
-      host_plan.size_segments = table->d_segments;
-      host_plan.tile_map = tile_map;
-      host_plan.chunk_row_start = reinterpret_cast<const unsigned long long*>(table->d_chunk_row_start);
-      host_plan.tile_count = tile_count;
+      target->raw_nulls[c] += host[layout.raw_nulls + at];
+      target->product_nulls[c] += host[layout.product_nulls + at];
+    }
+  }
+  if (!consistent) return false;
+  for (const auto& m : merged) {
+    HostGroup group;
+    group.key = m.key;
+    group.null_mask = m.null_mask;
+    group.rows = m.rows;
+    group.min_position = m.min_position;
+    group.max_position = m.max_position;
+    group.accumulators.assign(query->aggregate_count, 0);
+    group.counts.assign(query->aggregate_count, 0);
+    for (uint32_t a = 0; a < query->aggregate_count; ++a) {
+      const auto& mapping = fast.mapping[a];
+      if (mapping.is_count_star) {
+        group.counts[a] = m.rows;
+        continue;
+      }
+      const uint32_t slot = mapping.column_slot;
+      const uint64_t nulls = mapping.uses_product ? m.product_nulls[slot] : m.raw_nulls[slot];
+      group.counts[a] = m.rows - nulls;
+      if (fast.work_type == 2) {
+        const int64_t sum = m.raw_i[slot];
+        std::memcpy(&group.accumulators[a], &sum, sizeof(sum));
+      } else {
+        const double sum = mapping.uses_product ? m.product_f[slot] : m.raw_f[slot];
+        std::memcpy(&group.accumulators[a], &sum, sizeof(sum));
+      }
+    }
+    groups->push_back(std::move(group));
+  }
+  return true;
+}
 
-      host_plan.predicate_count = query->predicate_count;
-      for (uint32_t p = 0; p < query->predicate_count; ++p) {
-        host_plan.predicate_segments[p] = table->d_segments + size_t{query->predicates[p].column_id} * chunk_count;
-        host_plan.predicate_tests[p] = tests[p];
-      }
-      host_plan.groupby_count = query->groupby_count;
-      for (uint32_t g = 0; g < query->groupby_count; ++g) {
-        host_plan.group_segments[g] = table->d_segments + size_t{query->groupby_column_ids[g]} * chunk_count;
-      }
-      for (size_t c = 0; c < fast.columns.size(); ++c) {
-        host_plan.value_segments[c] = table->d_segments + size_t{fast.columns[c].column} * chunk_count;
-        host_plan.affine_kind[c] = fast.columns[c].kind;
-        host_plan.literal[c] = fast.columns[c].literal;
-      }
-      host_plan.need_raw_mask = fast.need_raw_mask;
-      host_plan.need_product_mask = fast.need_product_mask;
-      const size_t entries = size_t{grid} * G;
-      // partials, the 32-bit NULL masks (two per word) and the overflow word: the copy back to the host covers all of them
-      const size_t words = entries * (1 + kMaxKeyWords + 3 + 4 * C) + (entries + 1) / 2 + 1;
-      void* scratch = nullptr;
-      HYB_TRY(device_alloc(context, sizeof(uint64_t) * words + sizeof(FastPlan) + 64, &scratch));
-      HYB_CUDA(cudaMemsetAsync(scratch, 0, sizeof(uint64_t) * words + sizeof(FastPlan) + 64, stream));
-      auto* cursor = static_cast<unsigned long long*>(scratch);
-      host_plan.partial_hash = cursor;
-      cursor += entries;
-      host_plan.partial_keys = cursor;
-      cursor += entries * kMaxKeyWords;
-      host_plan.partial_rows = cursor;
-      cursor += entries;
-      host_plan.partial_min_position = cursor;
-      cursor += entries;
-      host_plan.partial_max_position = cursor;
-      cursor += entries;
-      host_plan.partial_raw = cursor;
-      cursor += entries * C;
-      host_plan.partial_product = cursor;
-      cursor += entries * C;
-      host_plan.partial_raw_nulls = cursor;
-      cursor += entries * C;
-      host_plan.partial_product_nulls = cursor;
-      cursor += entries * C;
-      host_plan.partial_null_mask = reinterpret_cast<uint32_t*>(cursor);
-      cursor += (entries + 1) / 2;
-      host_plan.overflow = reinterpret_cast<uint32_t*>(cursor);
-      cursor += 1;
-      auto* device_plan = reinterpret_cast<FastPlan*>(cursor);
+// The low-cardinality kernels over unfiltered inputs. Attempts in order: the TMA-staged streaming kernel when the layout
+// allows it (<= 4 groups), then the register-tile kernel with 4 and 8 group slots; a kernel that meets more groups than
+// it has slots raises `overflow`. out->done stays false when no attempt holds the groups or two groups share a hash.
+static int run_fast_path(hyb_context* context, Table* table, const hyb_aggregate_query* query, const FusedPredicates& fused,
+                         AggregatePlanMemo* memo, AggregateOutcome* out) {
+  const FastPlanHost fast = plan_fast_path(table, query);
+  const uint32_t chunk_count = table->chunk_count();
+  if (!fast.possible || chunk_count == 0) return HYB_OK;
+  cudaStream_t stream = context->stream;
+  const int C = fast.columns.size() <= 1 ? 1 : fast.columns.size() <= 2 ? 2 : 4;
+  struct Attempt {
+    bool stream;
+    int groups;
+  };
+  std::vector<Attempt> attempts;
+  StreamLayout stream_layout;
+  if (context->options.aggregate_stream) {
+    if (!memo->has_stream_layout || memo->stream_stages != context->options.aggregate_stages) {
+      memo->stream_layout = stream_layout_for(table, query, fast, context->options.aggregate_stages, fused.tree != nullptr);
+      memo->stream_stages = context->options.aggregate_stages;
+      memo->has_stream_layout = true;
+    }
+    stream_layout = memo->stream_layout;
+  }
+  if (stream_layout.possible) attempts.push_back({true, query->groupby_count == 0 ? 1 : 4});
+  if (query->groupby_count == 0) {
+    attempts.push_back({false, 1});
+  } else {
+    attempts.push_back({false, 4});
+    attempts.push_back({false, 8});
+  }
+  for (const Attempt attempt : attempts) {
+    const uint2* tile_map = nullptr;
+    uint32_t tile_count = 0;
+    HYB_TRY(get_tile_map(context, table, attempt.stream ? kStreamTileRows : kAggTileRows, &tile_map, &tile_count));
+    const int G = attempt.groups;
+    const FastKernel kernel = fast_kernel(fast.work_type, G, C, fused.tree != nullptr);
+    uint32_t grid = 1;
+    if (attempt.stream) {
+      // one persistent CTA per SM; its tiles are kStreamRounds contiguous runs, the runs strided over the CTAs
+      grid = std::max<uint32_t>(1, std::min<uint32_t>(tile_count, context->sm_count));
+    } else {
+      int blocks_per_sm = 1;
+      HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kernel, kFastThreads, 0));
+      // one wave of resident CTAs: the static tile striding must not queue CTAs behind each other
+      grid = std::max<uint32_t>(1, std::min<uint32_t>(tile_count, context->sm_count * std::max(blocks_per_sm, 1)));
+    }
+    FastPlan host_plan{};
+    plan_inputs(table, query, fused, &host_plan);
+    host_plan.size_segments = table->d_segments;
+    host_plan.tile_map = tile_map;
+    host_plan.tile_count = tile_count;
+    for (size_t c = 0; c < fast.columns.size(); ++c) {
+      host_plan.value_segments[c] = table->d_segments + size_t{fast.columns[c].column} * chunk_count;
+      host_plan.affine_kind[c] = fast.columns[c].kind;
+      host_plan.literal[c] = fast.columns[c].literal;
+    }
+    host_plan.need_raw_mask = fast.need_raw_mask;
+    host_plan.need_product_mask = fast.need_product_mask;
+    const size_t entries = size_t{grid} * G;
+    const FastPartials layout(entries, C);
+    std::vector<uint64_t> host(layout.words);
+    {
+      DeviceScratch scratch(context);  // this attempt's partials and plan
+      const size_t bytes = sizeof(uint64_t) * layout.words + sizeof(FastPlan) + 64;
+      void* block = nullptr;
+      HYB_TRY(scratch.alloc(bytes, &block));
+      HYB_CUDA(cudaMemsetAsync(block, 0, bytes, stream));
+      auto* partials = static_cast<unsigned long long*>(block);
+      host_plan.partial_hash = partials + layout.hash;
+      host_plan.partial_keys = partials + layout.keys;
+      host_plan.partial_rows = partials + layout.rows;
+      host_plan.partial_min_position = partials + layout.min_position;
+      host_plan.partial_max_position = partials + layout.max_position;
+      host_plan.partial_raw = partials + layout.raw;
+      host_plan.partial_product = partials + layout.product;
+      host_plan.partial_raw_nulls = partials + layout.raw_nulls;
+      host_plan.partial_product_nulls = partials + layout.product_nulls;
+      host_plan.partial_null_mask = reinterpret_cast<uint32_t*>(partials + layout.null_mask);
+      host_plan.overflow = reinterpret_cast<uint32_t*>(partials + layout.overflow);
+      auto* device_plan = reinterpret_cast<FastPlan*>(partials + layout.words);
       if (attempt.stream) {
         StreamPlan stream_plan = stream_layout.plan;
         stream_plan.fast = host_plan;
@@ -2203,267 +2257,234 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
         timing_kernel_begin(context);
         HYB_CUDA(cudaLaunchKernel(stream_kernel, dim3(grid), dim3(kStreamThreads), arguments, stream_layout.dynamic_bytes, stream));
         timing_kernel_end(context);
-        path = static_shape ? HYB_AGG_PATH_STREAM_STATIC : HYB_AGG_PATH_STREAM_GENERIC;
+        out->path = static_shape ? HYB_AGG_PATH_STREAM_STATIC : HYB_AGG_PATH_STREAM_GENERIC;
       } else {
-      HYB_CUDA(cudaMemcpyAsync(device_plan, &host_plan, sizeof(FastPlan), cudaMemcpyHostToDevice, stream));
-      void* arguments[] = {&device_plan, &tree_program};  // aggregate_fast_kernel takes the first only
-      timing_kernel_begin(context);
-      HYB_CUDA(cudaLaunchKernel(kernel, dim3(grid), dim3(kFastThreads), arguments, 0, stream));
-      timing_kernel_end(context);
-      path = G <= 4 ? HYB_AGG_PATH_TILE_G4 : HYB_AGG_PATH_TILE_G8;
+        HYB_CUDA(cudaMemcpyAsync(device_plan, &host_plan, sizeof(FastPlan), cudaMemcpyHostToDevice, stream));
+        const TestProgram* tree_program = fused.tree;
+        void* arguments[] = {&device_plan, &tree_program};  // aggregate_fast_kernel takes the first only
+        timing_kernel_begin(context);
+        HYB_CUDA(cudaLaunchKernel(kernel, dim3(grid), dim3(kFastThreads), arguments, 0, stream));
+        timing_kernel_end(context);
+        out->path = G <= 4 ? HYB_AGG_PATH_TILE_G4 : HYB_AGG_PATH_TILE_G8;
       }
-      kernel_timed = true;
+      out->kernel_timed = true;
       HYB_CUDA(cudaGetLastError());
-      ++launches;
-      std::vector<uint64_t> host(words);
-      HYB_CUDA(cudaMemcpyAsync(host.data(), scratch, sizeof(uint64_t) * words, cudaMemcpyDeviceToHost, stream));
+      ++out->launches;
+      HYB_CUDA(cudaMemcpyAsync(host.data(), block, sizeof(uint64_t) * layout.words, cudaMemcpyDeviceToHost, stream));
       HYB_CUDA(cudaStreamSynchronize(stream));
-      device_free(context, scratch);
-      const auto offset_of = [&](const void* pointer) {
-        return static_cast<size_t>(static_cast<const unsigned long long*>(pointer) - static_cast<unsigned long long*>(scratch));
-      };
-      const uint32_t overflow = *reinterpret_cast<const uint32_t*>(&host[offset_of(host_plan.overflow)]);
-      if (overflow) continue;  // more groups than this instantiation holds
-      // merge the per-CTA partials in CTA order (deterministic)
-      const uint64_t* p_hash = &host[offset_of(host_plan.partial_hash)];
-      const uint64_t* p_keys = &host[offset_of(host_plan.partial_keys)];
-      const uint64_t* p_rows = &host[offset_of(host_plan.partial_rows)];
-      const uint64_t* p_min = &host[offset_of(host_plan.partial_min_position)];
-      const uint64_t* p_max = &host[offset_of(host_plan.partial_max_position)];
-      const uint64_t* p_raw = &host[offset_of(host_plan.partial_raw)];
-      const uint64_t* p_product = &host[offset_of(host_plan.partial_product)];
-      const uint64_t* p_raw_nulls = &host[offset_of(host_plan.partial_raw_nulls)];
-      const uint64_t* p_product_nulls = &host[offset_of(host_plan.partial_product_nulls)];
-      const uint32_t* p_null_mask = reinterpret_cast<const uint32_t*>(&host[offset_of(host_plan.partial_null_mask)]);
-      struct Merged {
-        uint64_t hash;
-        std::vector<uint64_t> key;
-        uint32_t null_mask;
-        uint64_t rows = 0, min_position = ~uint64_t{0}, max_position = 0;
-        std::vector<double> raw_f, product_f;
-        std::vector<int64_t> raw_i;
-        std::vector<uint64_t> raw_nulls, product_nulls;
-      };
-      std::vector<Merged> merged;
-      bool consistent = true;
-      for (size_t entry = 0; entry < entries; ++entry) {
-        if (p_hash[entry] == 0 || p_rows[entry] == 0) continue;
-        std::vector<uint64_t> key(p_keys + entry * kMaxKeyWords, p_keys + entry * kMaxKeyWords + std::max<uint32_t>(query->groupby_count, 1));
-        Merged* target = nullptr;
-        for (auto& m : merged) {
-          if (m.hash == p_hash[entry]) {
-            if (m.key != key || m.null_mask != p_null_mask[entry]) consistent = false;  // 64-bit hash collision
-            target = &m;
-          }
-        }
-        if (!target) {
-          merged.emplace_back();
-          target = &merged.back();
-          target->hash = p_hash[entry];
-          target->key = key;
-          target->null_mask = p_null_mask[entry];
-          target->raw_f.assign(C, 0.0);
-          target->product_f.assign(C, 0.0);
-          target->raw_i.assign(C, 0);
-          target->raw_nulls.assign(C, 0);
-          target->product_nulls.assign(C, 0);
-        }
-        target->rows += p_rows[entry];
-        target->min_position = std::min(target->min_position, p_min[entry]);
-        target->max_position = std::max(target->max_position, p_max[entry]);
-        for (int c = 0; c < C; ++c) {
-          if (fast.work_type == 2) {
-            target->raw_i[c] += static_cast<int64_t>(p_raw[entry * C + c]);
-          } else {
-            double raw, product;
-            std::memcpy(&raw, &p_raw[entry * C + c], sizeof(double));
-            std::memcpy(&product, &p_product[entry * C + c], sizeof(double));
-            target->raw_f[c] += raw;
-            target->product_f[c] += product;
-          }
-          target->raw_nulls[c] += p_raw_nulls[entry * C + c];
-          target->product_nulls[c] += p_product_nulls[entry * C + c];
+    }
+    const uint32_t overflow = *reinterpret_cast<const uint32_t*>(&host[layout.overflow]);
+    if (overflow) continue;  // more groups than this instantiation holds
+    out->done = merge_fast_partials(query, fast, host, layout, entries, C, &out->groups);
+    break;  // a hash collision falls through to the general path
+  }
+  return HYB_OK;
+}
+
+// One sweep of aggregate_general_kernel over the plan's rows; with an expression tree, its kTreeRows form.
+template <int kSweep>
+static void launch_general_sweep(bool tree, uint32_t grid, cudaStream_t stream, const AggregatePlan* plan,
+                                 const GroupTable& group_table, const GroupTable& distinct_table) {
+  if (tree) {
+    aggregate_general_kernel<kSweep | kTreeRows><<<grid, kAggThreads, 0, stream>>>(plan, group_table, distinct_table);
+  } else {
+    aggregate_general_kernel<kSweep><<<grid, kAggThreads, 0, stream>>>(plan, group_table, distinct_table);
+  }
+}
+
+// The groups of aggregate_compact_kernel's packed copy of `slots` slots; MIN / MAX and STDDEV_SAMP get their values.
+static void parse_packed_groups(const hyb_aggregate_query* query, const AggregateTypes& types, const uint64_t* words,
+                                uint64_t slots, uint32_t key_words, size_t compact_words, std::vector<HostGroup>* groups) {
+  const uint32_t aggregate_count = query->aggregate_count;
+  const uint64_t* h_hashes = words;
+  const uint64_t* h_keys = h_hashes + slots;
+  const uint64_t* h_rows = h_keys + slots * key_words;
+  const uint64_t* h_min = h_rows + slots;
+  const uint64_t* h_max = h_min + slots;
+  const uint64_t* h_acc = h_max + slots;
+  const uint64_t* h_counts = h_acc + slots * aggregate_count;
+  const uint64_t* h_zero_first = h_counts + slots * aggregate_count;
+  const uint64_t* h_moments = h_zero_first + slots * aggregate_count;  // STDDEV_SAMP plans: {Σd, Σd²} per aggregate
+  const uint32_t* h_null_masks = reinterpret_cast<const uint32_t*>(words + compact_words);
+  for (uint64_t slot = 0; slot < slots; ++slot) {
+    if (h_hashes[slot] == 0) continue;
+    HostGroup group;
+    group.key.assign(h_keys + slot * key_words, h_keys + (slot + 1) * key_words);
+    group.null_mask = h_null_masks[slot];
+    group.rows = h_rows[slot];
+    group.min_position = h_min[slot];
+    group.max_position = h_max[slot];
+    group.accumulators.resize(aggregate_count);
+    group.counts.resize(aggregate_count);
+    for (uint32_t a = 0; a < aggregate_count; ++a) {
+      group.accumulators[a] = h_acc[size_t{a} * slots + slot];
+      group.counts[a] = query->aggregates[a].function == HYB_AGG_COUNT_STAR ? group.rows : h_counts[size_t{a} * slots + slot];
+      const int32_t function = query->aggregates[a].function;
+      if (function == HYB_AGG_STDDEV_SAMP && group.counts[a] > 1) {
+        // M2 = Σd² - (Σd)² / n; rounding may leave it a hair below 0 where Welford's M2 cannot go. Only a negative M2
+        // is clamped: a NaN (a NaN or an infinity in the group) stays NaN, as in the reference's Welford.
+        double sum_d, sum_d2;
+        std::memcpy(&sum_d, h_moments + (size_t{a} * 2) * slots + slot, sizeof(double));
+        std::memcpy(&sum_d2, h_moments + (size_t{a} * 2 + 1) * slots + slot, sizeof(double));
+        const double n = static_cast<double>(group.counts[a]);
+        double m2 = sum_d2 - sum_d * sum_d / n;
+        if (m2 < 0.0) m2 = 0.0;
+        const double deviation = std::sqrt(m2 / (n - 1.0));
+        std::memcpy(&group.accumulators[a], &deviation, sizeof(deviation));
+      }
+      const int32_t input_type = types.input_types[a];
+      if ((function == HYB_AGG_MIN || function == HYB_AGG_MAX) && group.counts[a] > 0 && input_type != HYB_TYPE_STRING) {
+        if (input_type == HYB_TYPE_INT32 || input_type == HYB_TYPE_INT64) {
+          group.accumulators[a] ^= 0x8000000000000000ull;
+        } else {
+          double value = double_from_ordered(group.accumulators[a]);
+          if (value == 0.0 && (h_zero_first[size_t{a} * slots + slot] & 1)) value = -0.0;  // the first zero was -0.0
+          std::memcpy(&group.accumulators[a], &value, sizeof(value));
         }
       }
-      if (!consistent) break;  // fall through to the general path
-      for (const auto& m : merged) {
-        HostGroup group;
-        group.key = m.key;
-        group.null_mask = m.null_mask;
-        group.rows = m.rows;
-        group.min_position = m.min_position;
-        group.max_position = m.max_position;
-        group.accumulators.assign(aggregate_count, 0);
-        group.counts.assign(aggregate_count, 0);
-        for (uint32_t a = 0; a < aggregate_count; ++a) {
-          const auto& mapping = fast.mapping[a];
-          if (mapping.is_count_star) {
-            group.counts[a] = m.rows;
-            continue;
-          }
-          const uint32_t slot = mapping.column_slot;
-          const uint64_t nulls = mapping.uses_product ? m.product_nulls[slot] : m.raw_nulls[slot];
-          group.counts[a] = m.rows - nulls;
-          if (fast.work_type == 2) {
-            const int64_t sum = m.raw_i[slot];
-            std::memcpy(&group.accumulators[a], &sum, sizeof(sum));
-          } else {
-            const double sum = mapping.uses_product ? m.product_f[slot] : m.raw_f[slot];
-            std::memcpy(&group.accumulators[a], &sum, sizeof(sum));
-          }
+    }
+    groups->push_back(std::move(group));
+  }
+}
+
+// The hash table kernel over any input. Grows the group table (and the COUNT(DISTINCT) set) by 8x until the kernel
+// finds no overflow, then runs the STDDEV_SAMP and string MIN / MAX passes and packs the occupied slots for the host.
+static int run_general_path(hyb_context* context, Table* table, const hyb_aggregate_query* query, const PosList* filter,
+                            uint64_t position_count, const AggregateTypes& types, const FusedPredicates& fused,
+                            AggregateOutcome* out) {
+  cudaStream_t stream = context->stream;
+  const uint32_t aggregate_count = query->aggregate_count;
+  const bool tree = fused.tree != nullptr;
+  const uint32_t chunk_count = table->chunk_count();
+  AggregatePlan host_plan{};
+  if (filter) {
+    host_plan.filter = filter->d_row_ids;
+    host_plan.tile_count = static_cast<uint32_t>((position_count + kAggTileRows - 1) / kAggTileRows);
+  } else {
+    HYB_TRY(get_tile_map(context, table, kAggTileRows, &host_plan.tile_map, &host_plan.tile_count));
+  }
+  plan_inputs(table, query, fused, &host_plan);
+  host_plan.position_count = position_count;
+  host_plan.chunk_count = chunk_count;
+  if (query->groupby_count == 0) host_plan.group_segments[0] = table->d_segments;  // sizes chunks when nothing else does
+  host_plan.aggregate_count = aggregate_count;
+  host_plan.tree = fused.tree;
+  std::vector<uint32_t> plan_columns;
+  for (uint32_t a = 0; a < query->aggregate_count; ++a) {
+    const auto& def = query->aggregates[a];
+    auto& device_aggregate = host_plan.aggregates[a];
+    device_aggregate.function = def.function;
+    device_aggregate.node_count = def.function == HYB_AGG_COUNT_STAR ? 0 : def.node_count;
+    device_aggregate.input_type = types.input_types[a];
+    device_aggregate.result_type = types.result_types[a];
+    for (uint32_t n = 0; n < device_aggregate.node_count; ++n) {
+      auto& node = device_aggregate.nodes[n];
+      node.op = def.nodes[n].op;
+      node.literal_type = def.nodes[n].literal_type;
+      node.literal = def.nodes[n].literal;
+      if (node.op == HYB_EXPR_COLUMN) {
+        auto it = std::find(plan_columns.begin(), plan_columns.end(), def.nodes[n].column_id);
+        if (it == plan_columns.end()) {
+          plan_columns.push_back(def.nodes[n].column_id);
+          it = plan_columns.end() - 1;
         }
-        groups.push_back(std::move(group));
+        node.column = static_cast<uint32_t>(it - plan_columns.begin());
       }
-      done = true;
-      break;
     }
   }
+  HYB_CHECK(plan_columns.size() <= HYB_MAX_AGGREGATES * 4, HYB_ERR_UNSUPPORTED, "too many distinct aggregate columns");
+  host_plan.column_count = static_cast<uint32_t>(plan_columns.size());
+  for (size_t c = 0; c < plan_columns.size(); ++c) {
+    host_plan.columns[c] = table->d_segments + size_t{plan_columns[c]} * chunk_count;
+  }
+  // a string column that a MIN / MAX / COUNT reads is its INT32 view for every aggregate of the plan (the view keeps
+  // the dictionary codes a COUNT(DISTINCT) of the same column reads)
+  StringExtremes string_extremes{};
+  bool has_string_extremes = false;
+  for (uint32_t a = 0; a < aggregate_count; ++a) {
+    if (!types.string_views[a]) continue;
+    host_plan.columns[host_plan.aggregates[a].nodes[0].column] = types.string_views[a]->d_segments;
+    if (types.result_types[a] == HYB_TYPE_STRING) {
+      string_extremes.first_entry[a] = types.string_views[a]->d_first_entry;
+      has_string_extremes = true;
+    }
+  }
+  DeviceScratch plan_scratch(context);
+  AggregatePlan* device_plan = nullptr;
+  HYB_TRY(plan_scratch.alloc_array(1, &device_plan));
+  HYB_CUDA(cudaMemcpyAsync(device_plan, &host_plan, sizeof(AggregatePlan), cudaMemcpyHostToDevice, stream));
+  HYB_CUDA(cudaStreamSynchronize(stream));  // host_plan is on the stack
 
-  // ---- general path -----------------------------------------------------------------------------------------------
-  if (!done) {
-    AggregatePlan host_plan{};
-    const uint2* tile_map = nullptr;
-    if (filter) {
-      host_plan.filter = filter->d_row_ids;
-      host_plan.tile_count = static_cast<uint32_t>((position_count + kAggTileRows - 1) / kAggTileRows);
-    } else {
-      HYB_TRY(get_tile_map(context, table, kAggTileRows, &tile_map, &host_plan.tile_count));
-      host_plan.tile_map = tile_map;
+  uint64_t capacity = 1024;
+  while (capacity < std::min<uint64_t>(position_count * 2, uint64_t{1} << 20)) capacity <<= 1;
+  uint64_t distinct_capacity = capacity;  // the COUNT(DISTINCT) set starts at the group table's size
+  const uint32_t key_words = std::max<uint32_t>(query->groupby_count, 1);
+  uint32_t distinct_mask = 0, stddev_mask = 0;
+  for (uint32_t a = 0; a < aggregate_count; ++a) {
+    if (query->aggregates[a].function == HYB_AGG_COUNT_DISTINCT) distinct_mask |= 1u << a;
+    if (query->aggregates[a].function == HYB_AGG_STDDEV_SAMP) stddev_mask |= 1u << a;
+  }
+  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>(host_plan.tile_count, context->sm_count * 8));
+  out->path = HYB_AGG_PATH_GENERAL;
+  while (!out->done) {
+    // more {group, value} pairs than a set of 2^31 slots holds at load factor 0.5: the CPU operator counts them
+    HYB_CHECK(distinct_capacity <= (uint64_t{1} << 31), HYB_ERR_UNSUPPORTED, "COUNT(DISTINCT) set would exceed 2^31 slots");
+    HYB_CHECK(capacity <= (uint64_t{1} << 31), HYB_ERR_OOM, "group table would exceed 2^31 slots");
+    // moments: {mean, Σd, Σd²} per aggregate and slot on the device; the packed copy carries {Σd, Σd²}
+    const size_t moment_words = stddev_mask ? 3 * size_t{aggregate_count} : 0;
+    const size_t per_slot_words = 1 + key_words + 3 + 3 * size_t{aggregate_count} + (stddev_mask ? 2 * size_t{aggregate_count} : 0);
+    const size_t bytes = sizeof(uint64_t) * capacity * (1 + key_words + 3 + 3 * size_t{aggregate_count} + moment_words) +
+                         sizeof(uint32_t) * capacity * 2 + 64;
+    DeviceScratch iteration(context);  // the group table and the compact buffer
+    void* table_block = nullptr;
+    HYB_TRY(iteration.alloc(bytes, &table_block));
+    HYB_CUDA(cudaMemsetAsync(table_block, 0, bytes, stream));
+    GroupTable group_table{};
+    group_table.capacity_mask = static_cast<uint32_t>(capacity - 1);
+    group_table.key_words = key_words;
+    auto* cursor = static_cast<unsigned long long*>(table_block);
+    group_table.hashes = cursor;
+    cursor += capacity;
+    group_table.keys = cursor;
+    cursor += capacity * key_words;
+    group_table.rows = cursor;
+    cursor += capacity;
+    group_table.min_position = cursor;
+    cursor += capacity;
+    group_table.max_position = cursor;
+    cursor += capacity;
+    group_table.accumulators = cursor;
+    cursor += capacity * aggregate_count;
+    group_table.counts = cursor;
+    cursor += capacity * aggregate_count;
+    group_table.zero_first = cursor;
+    cursor += capacity * aggregate_count;
+    if (stddev_mask) {
+      group_table.moments = reinterpret_cast<double*>(cursor);
+      cursor += capacity * moment_words;
     }
-    host_plan.chunk_row_start = reinterpret_cast<const unsigned long long*>(table->d_chunk_row_start);
-    host_plan.position_count = position_count;
-    host_plan.chunk_count = chunk_count;
-    host_plan.predicate_count = query->predicate_count;
-    for (uint32_t p = 0; p < query->predicate_count; ++p) {
-      host_plan.predicate_segments[p] = table->d_segments + size_t{query->predicates[p].column_id} * chunk_count;
-      host_plan.predicate_tests[p] = tests[p];
-    }
-    host_plan.groupby_count = query->groupby_count;
-    for (uint32_t g = 0; g < query->groupby_count; ++g) {
-      host_plan.group_segments[g] = table->d_segments + size_t{query->groupby_column_ids[g]} * chunk_count;
-    }
-    if (query->groupby_count == 0) host_plan.group_segments[0] = table->d_segments;  // sizes chunks when nothing else does
-    host_plan.aggregate_count = aggregate_count;
-    host_plan.tree = tree_program;
-    std::vector<uint32_t> plan_columns;
-    for (uint32_t a = 0; a < aggregate_count; ++a) {
-      const auto& def = query->aggregates[a];
-      auto& device_aggregate = host_plan.aggregates[a];
-      device_aggregate.function = def.function;
-      device_aggregate.node_count = def.function == HYB_AGG_COUNT_STAR ? 0 : def.node_count;
-      device_aggregate.input_type = input_types[a];
-      device_aggregate.result_type = result_types[a];
-      for (uint32_t n = 0; n < device_aggregate.node_count; ++n) {
-        auto& node = device_aggregate.nodes[n];
-        node.op = def.nodes[n].op;
-        node.literal_type = def.nodes[n].literal_type;
-        node.literal = def.nodes[n].literal;
-        if (node.op == HYB_EXPR_COLUMN) {
-          auto it = std::find(plan_columns.begin(), plan_columns.end(), def.nodes[n].column_id);
-          if (it == plan_columns.end()) {
-            plan_columns.push_back(def.nodes[n].column_id);
-            it = plan_columns.end() - 1;
-          }
-          node.column = static_cast<uint32_t>(it - plan_columns.begin());
-        }
-      }
-    }
-    HYB_CHECK(plan_columns.size() <= HYB_MAX_AGGREGATES * 4, HYB_ERR_UNSUPPORTED, "too many distinct aggregate columns");
-    host_plan.column_count = static_cast<uint32_t>(plan_columns.size());
-    for (size_t c = 0; c < plan_columns.size(); ++c) {
-      host_plan.columns[c] = table->d_segments + size_t{plan_columns[c]} * chunk_count;
-    }
-    // a string column that a MIN / MAX / COUNT reads is its INT32 view for every aggregate of the plan (the view keeps
-    // the dictionary codes a COUNT(DISTINCT) of the same column reads)
-    StringExtremes string_extremes{};
-    bool has_string_extremes = false;
-    for (uint32_t a = 0; a < aggregate_count; ++a) {
-      if (!string_views[a]) continue;
-      host_plan.columns[host_plan.aggregates[a].nodes[0].column] = string_views[a]->d_segments;
-      if (result_types[a] == HYB_TYPE_STRING) {
-        string_extremes.first_entry[a] = string_views[a]->d_first_entry;
-        has_string_extremes = true;
-      }
-    }
-    void* device_plan = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(AggregatePlan), &device_plan));
-    HYB_CUDA(cudaMemcpyAsync(device_plan, &host_plan, sizeof(AggregatePlan), cudaMemcpyHostToDevice, stream));
-    HYB_CUDA(cudaStreamSynchronize(stream));  // host_plan is on the stack
-
-    uint64_t capacity = 1024;
-    while (capacity < std::min<uint64_t>(position_count * 2, uint64_t{1} << 20)) capacity <<= 1;
-    uint64_t distinct_capacity = capacity;  // the COUNT(DISTINCT) set starts at the group table's size
-    const uint32_t key_words = std::max<uint32_t>(query->groupby_count, 1);
-    uint32_t distinct_mask = 0, stddev_mask = 0;
-    for (uint32_t a = 0; a < aggregate_count; ++a) {
-      if (query->aggregates[a].function == HYB_AGG_COUNT_DISTINCT) distinct_mask |= 1u << a;
-      if (query->aggregates[a].function == HYB_AGG_STDDEV_SAMP) stddev_mask |= 1u << a;
-    }
-    path = HYB_AGG_PATH_GENERAL;
-    const auto release_general = [&]() {
-      device_free(context, device_plan);
-      release_tests();
-    };
-    while (!done) {
-      if (distinct_capacity > (uint64_t{1} << 31)) {
-        // more {group, value} pairs than a set of 2^31 slots holds at load factor 0.5: the CPU operator counts them
-        release_general();
-        HYB_CHECK(false, HYB_ERR_UNSUPPORTED, "COUNT(DISTINCT) set would exceed 2^31 slots");
-      }
-      HYB_CHECK(capacity <= (uint64_t{1} << 31), HYB_ERR_OOM, "group table would exceed 2^31 slots");
-      // moments: {mean, Σd, Σd²} per aggregate and slot on the device; the packed copy carries {Σd, Σd²}
-      const size_t moment_words = stddev_mask ? 3 * size_t{aggregate_count} : 0;
-      const size_t per_slot_words = 1 + key_words + 3 + 3 * size_t{aggregate_count} + (stddev_mask ? 2 * size_t{aggregate_count} : 0);
-      const size_t bytes = sizeof(uint64_t) * capacity * (1 + key_words + 3 + 3 * size_t{aggregate_count} + moment_words) +
-                           sizeof(uint32_t) * capacity * 2 + 64;
-      void* scratch = nullptr;
-      HYB_TRY(device_alloc(context, bytes, &scratch));
-      HYB_CUDA(cudaMemsetAsync(scratch, 0, bytes, stream));
-      // The COUNT(DISTINCT) set: hashes, {aggregate << 32 | group slot, value word} keys, states and its control words.
-      GroupTable distinct_table{};
-      void* distinct_scratch = nullptr;
+    group_table.states = reinterpret_cast<uint32_t*>(cursor);
+    group_table.null_masks = group_table.states + capacity;
+    group_table.control = group_table.null_masks + capacity;
+    // {groups inserted, overflow} of both tables: these words decide whether the tables were big enough
+    uint32_t table_control[2] = {0, 0}, distinct_control[2] = {0, 0};
+    // The COUNT(DISTINCT) set: hashes, {aggregate << 32 | group slot, value word} keys, states and its control words.
+    // Only the first sweep reads it; it is freed once its control words are read.
+    GroupTable distinct_table{};
+    {
+      DeviceScratch distinct_scratch(context);
       if (distinct_mask) {
         const size_t distinct_bytes = sizeof(uint64_t) * distinct_capacity * 3 + sizeof(uint32_t) * distinct_capacity + 64;
-        if (const int status = device_alloc(context, distinct_bytes, &distinct_scratch); status != HYB_OK) {
-          device_free(context, scratch);
-          release_general();
-          return status;
-        }
-        HYB_CUDA(cudaMemsetAsync(distinct_scratch, 0, distinct_bytes, stream));
+        void* distinct_block = nullptr;
+        HYB_TRY(distinct_scratch.alloc(distinct_bytes, &distinct_block));
+        HYB_CUDA(cudaMemsetAsync(distinct_block, 0, distinct_bytes, stream));
         distinct_table.capacity_mask = static_cast<uint32_t>(distinct_capacity - 1);
         distinct_table.key_words = 2;
-        distinct_table.hashes = static_cast<unsigned long long*>(distinct_scratch);
+        distinct_table.hashes = static_cast<unsigned long long*>(distinct_block);
         distinct_table.keys = distinct_table.hashes + distinct_capacity;
         distinct_table.states = reinterpret_cast<uint32_t*>(distinct_table.keys + distinct_capacity * 2);
         distinct_table.control = distinct_table.states + distinct_capacity;
       }
-      GroupTable group_table{};
-      group_table.capacity_mask = static_cast<uint32_t>(capacity - 1);
-      group_table.key_words = key_words;
-      auto* cursor = static_cast<unsigned long long*>(scratch);
-      group_table.hashes = cursor;
-      cursor += capacity;
-      group_table.keys = cursor;
-      cursor += capacity * key_words;
-      group_table.rows = cursor;
-      cursor += capacity;
-      group_table.min_position = cursor;
-      cursor += capacity;
-      group_table.max_position = cursor;
-      cursor += capacity;
-      group_table.accumulators = cursor;
-      cursor += capacity * aggregate_count;
-      group_table.counts = cursor;
-      cursor += capacity * aggregate_count;
-      group_table.zero_first = cursor;
-      cursor += capacity * aggregate_count;
-      if (stddev_mask) {
-        group_table.moments = reinterpret_cast<double*>(cursor);
-        cursor += capacity * moment_words;
-      }
-      group_table.states = reinterpret_cast<uint32_t*>(cursor);
-      group_table.null_masks = group_table.states + capacity;
-      group_table.control = group_table.null_masks + capacity;
       HYB_CUDA(cudaMemsetAsync(group_table.min_position, 0xFF, sizeof(uint64_t) * capacity, stream));
       for (uint32_t a = 0; a < aggregate_count; ++a) {
         if (query->aggregates[a].function == HYB_AGG_MIN) {
@@ -2473,159 +2494,82 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
           HYB_CUDA(cudaMemsetAsync(group_table.zero_first + size_t{a} * capacity, 0xFF, sizeof(uint64_t) * capacity, stream));
         }
       }
-      const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>(host_plan.tile_count, context->sm_count * 8));
-      if (!kernel_timed) timing_kernel_begin(context);
-      const auto* plan_arg = static_cast<const AggregatePlan*>(device_plan);
+      if (!out->kernel_timed) timing_kernel_begin(context);
       if (host_plan.tile_count) {
-        if (tree && (distinct_mask || stddev_mask)) {
-          aggregate_general_kernel<kWithDistinct | kTreeRows><<<grid, kAggThreads, 0, stream>>>(plan_arg, group_table,
-                                                                                                 distinct_table);
-        } else if (tree) {
-          aggregate_general_kernel<kPlain | kTreeRows><<<grid, kAggThreads, 0, stream>>>(plan_arg, group_table, distinct_table);
-        } else if (distinct_mask || stddev_mask) {
-          aggregate_general_kernel<kWithDistinct><<<grid, kAggThreads, 0, stream>>>(plan_arg, group_table, distinct_table);
+        if (distinct_mask || stddev_mask) {
+          launch_general_sweep<kWithDistinct>(tree, grid, stream, device_plan, group_table, distinct_table);
         } else {
-          aggregate_general_kernel<kPlain><<<grid, kAggThreads, 0, stream>>>(plan_arg, group_table, distinct_table);
+          launch_general_sweep<kPlain>(tree, grid, stream, device_plan, group_table, distinct_table);
         }
         HYB_CUDA(cudaGetLastError());
-        ++launches;
+        ++out->launches;
       }
-      if (!kernel_timed) timing_kernel_end(context);
-      kernel_timed = true;
-      // {groups inserted, overflow} of both tables: these words decide whether the tables were big enough
-      uint32_t table_control[2] = {0, 0}, distinct_control[2] = {0, 0};
+      if (!out->kernel_timed) timing_kernel_end(context);
+      out->kernel_timed = true;
       HYB_CUDA(cudaMemcpyAsync(table_control, group_table.control, sizeof(table_control), cudaMemcpyDeviceToHost, stream));
       if (distinct_mask) {
         HYB_CUDA(cudaMemcpyAsync(distinct_control, distinct_table.control, sizeof(distinct_control), cudaMemcpyDeviceToHost,
                                  stream));
       }
       HYB_CUDA(cudaStreamSynchronize(stream));
-      if (distinct_scratch) device_free(context, distinct_scratch);
-      if (table_control[1] || distinct_control[1]) {
-        device_free(context, scratch);
-        if (table_control[1]) capacity <<= 3;
-        if (distinct_control[1]) distinct_capacity <<= 3;
-        path = HYB_AGG_PATH_GENERAL_REGROWN;
-        continue;
-      }
-      if (stddev_mask && table_control[0]) {
-        // corrected two-pass variance: the means, then the deviations of the same rows from them
-        const uint32_t slot_grid =
-            static_cast<uint32_t>(std::min<uint64_t>((capacity + 255) / 256, static_cast<uint64_t>(context->sm_count) * 16));
-        timing_kernel_begin(context);
-        stddev_mean_kernel<<<slot_grid, 256, 0, stream>>>(group_table, aggregate_count, stddev_mask);
-        HYB_CUDA(cudaGetLastError());
-        if (tree) {  // the same rows as the first sweep
-          aggregate_general_kernel<kDeviations | kTreeRows><<<grid, kAggThreads, 0, stream>>>(plan_arg, group_table,
-                                                                                               distinct_table);
-        } else {
-          aggregate_general_kernel<kDeviations><<<grid, kAggThreads, 0, stream>>>(plan_arg, group_table, distinct_table);
-        }
-        HYB_CUDA(cudaGetLastError());
-        timing_kernel_end(context);
-        launches += 2;
-      }
-      if (has_string_extremes && table_control[0]) {
-        const uint32_t slot_grid =
-            static_cast<uint32_t>(std::min<uint64_t>((capacity + 255) / 256, static_cast<uint64_t>(context->sm_count) * 16));
-        string_extreme_kernel<<<slot_grid, 256, 0, stream>>>(group_table, aggregate_count, string_extremes);
-        HYB_CUDA(cudaGetLastError());
-        ++launches;
-      }
-      // pack the occupied slots on the device; only they travel to the host
-      const uint64_t group_slots = table_control[0];
-      const size_t compact_words = std::max<uint64_t>(group_slots, 1) * per_slot_words;
-      const size_t compact_bytes = sizeof(uint64_t) * compact_words + sizeof(uint32_t) * std::max<uint64_t>(group_slots, 1) + 64;
-      void* compact = nullptr;
-      HYB_TRY(device_alloc(context, compact_bytes, &compact));
-      auto* compact_null_masks = reinterpret_cast<uint32_t*>(static_cast<unsigned long long*>(compact) + compact_words);
-      uint32_t* compact_cursor = compact_null_masks + std::max<uint64_t>(group_slots, 1);
-      HYB_CUDA(cudaMemsetAsync(compact_cursor, 0, sizeof(uint32_t), stream));
-      if (group_slots) {
-        const uint32_t compact_grid = static_cast<uint32_t>(std::min<uint64_t>((capacity + 255) / 256, uint64_t{context->sm_count} * 16));
-        aggregate_compact_kernel<<<compact_grid, 256, 0, stream>>>(group_table, aggregate_count, static_cast<uint32_t>(group_slots),
-                                                                   static_cast<unsigned long long*>(compact), compact_null_masks,
-                                                                   compact_cursor);
-        HYB_CUDA(cudaGetLastError());
-        ++launches;
-      }
-      std::vector<uint8_t> host(compact_bytes);
-      HYB_CUDA(cudaMemcpyAsync(host.data(), compact, compact_bytes, cudaMemcpyDeviceToHost, stream));
-      HYB_CUDA(cudaStreamSynchronize(stream));
-      device_free(context, compact);
-      device_free(context, scratch);
-      const auto* words = reinterpret_cast<const uint64_t*>(host.data());
-      const uint64_t table_capacity = capacity;
-      capacity = group_slots;  // the parsing below walks the packed arrays
-      const uint64_t* h_hashes = words;
-      const uint64_t* h_keys = h_hashes + capacity;
-      const uint64_t* h_rows = h_keys + capacity * key_words;
-      const uint64_t* h_min = h_rows + capacity;
-      const uint64_t* h_max = h_min + capacity;
-      const uint64_t* h_acc = h_max + capacity;
-      const uint64_t* h_counts = h_acc + capacity * aggregate_count;
-      const uint64_t* h_zero_first = h_counts + capacity * aggregate_count;
-      const uint64_t* h_moments = h_zero_first + capacity * aggregate_count;  // STDDEV_SAMP plans: {Σd, Σd²} per aggregate
-      const uint32_t* h_null_masks = reinterpret_cast<const uint32_t*>(words + compact_words);
-      (void)table_capacity;
-      for (uint64_t slot = 0; slot < capacity; ++slot) {
-        if (h_hashes[slot] == 0) continue;
-        HostGroup group;
-        group.key.assign(h_keys + slot * key_words, h_keys + (slot + 1) * key_words);
-        group.null_mask = h_null_masks[slot];
-        group.rows = h_rows[slot];
-        group.min_position = h_min[slot];
-        group.max_position = h_max[slot];
-        group.accumulators.resize(aggregate_count);
-        group.counts.resize(aggregate_count);
-        for (uint32_t a = 0; a < aggregate_count; ++a) {
-          group.accumulators[a] = h_acc[size_t{a} * capacity + slot];
-          group.counts[a] = query->aggregates[a].function == HYB_AGG_COUNT_STAR ? group.rows : h_counts[size_t{a} * capacity + slot];
-          // undo the ordered encodings of MIN / MAX
-          const int32_t function = query->aggregates[a].function;
-          if (function == HYB_AGG_STDDEV_SAMP && group.counts[a] > 1) {
-            // M2 = Σd² - (Σd)² / n; rounding may leave it a hair below 0 where Welford's M2 cannot go. Only a negative M2
-            // is clamped: a NaN (a NaN or an infinity in the group) stays NaN, as in the reference's Welford.
-            double sum_d, sum_d2;
-            std::memcpy(&sum_d, h_moments + (size_t{a} * 2) * capacity + slot, sizeof(double));
-            std::memcpy(&sum_d2, h_moments + (size_t{a} * 2 + 1) * capacity + slot, sizeof(double));
-            const double n = static_cast<double>(group.counts[a]);
-            double m2 = sum_d2 - sum_d * sum_d / n;
-            if (m2 < 0.0) m2 = 0.0;
-            const double deviation = std::sqrt(m2 / (n - 1.0));
-            std::memcpy(&group.accumulators[a], &deviation, sizeof(deviation));
-          }
-          if ((function == HYB_AGG_MIN || function == HYB_AGG_MAX) && group.counts[a] > 0 && input_types[a] != HYB_TYPE_STRING) {
-            const bool integral = input_types[a] == HYB_TYPE_INT32 || input_types[a] == HYB_TYPE_INT64;
-            if (integral) {
-              group.accumulators[a] ^= 0x8000000000000000ull;
-            } else {
-              double value = double_from_ordered(group.accumulators[a]);
-              if (value == 0.0 && (h_zero_first[size_t{a} * capacity + slot] & 1)) value = -0.0;  // the first zero was -0.0
-              std::memcpy(&group.accumulators[a], &value, sizeof(value));
-            }
-          }
-        }
-        groups.push_back(std::move(group));
-      }
-      done = true;
     }
-    device_free(context, device_plan);
-  }
-  release_tests();
-
-  if (exchange) {
-    HYB_CHECK(!filter, HYB_ERR_UNSUPPORTED, "distributed aggregation of position-filtered inputs is not on the GPU path");
-    // Low cardinality: one 32 KB block per rank, replicated result. A rank whose partial groups do not fit sends its block's
-    // header alone; every rank sees that in the same set of blocks and all of them switch to the partitioned exchange.
-    bool needs_partitioning = false;
-    HYB_TRY(exchange_partial_groups(context, *exchange, table, query, input_types, &groups, &needs_partitioning));
-    if (needs_partitioning) {
-      HYB_TRY(exchange_partial_groups_partitioned(context, *exchange, table, query, input_types, &groups, &forced_immediate));
+    if (table_control[1] || distinct_control[1]) {
+      if (table_control[1]) capacity <<= 3;
+      if (distinct_control[1]) distinct_capacity <<= 3;
+      out->path = HYB_AGG_PATH_GENERAL_REGROWN;
+      continue;
     }
+    const uint32_t slot_grid =
+        static_cast<uint32_t>(std::min<uint64_t>((capacity + 255) / 256, static_cast<uint64_t>(context->sm_count) * 16));
+    if (stddev_mask && table_control[0]) {
+      // corrected two-pass variance: the means, then the deviations of the same rows from them
+      timing_kernel_begin(context);
+      stddev_mean_kernel<<<slot_grid, 256, 0, stream>>>(group_table, aggregate_count, stddev_mask);
+      HYB_CUDA(cudaGetLastError());
+      launch_general_sweep<kDeviations>(tree, grid, stream, device_plan, group_table, distinct_table);
+      HYB_CUDA(cudaGetLastError());
+      timing_kernel_end(context);
+      out->launches += 2;
+    }
+    if (has_string_extremes && table_control[0]) {
+      string_extreme_kernel<<<slot_grid, 256, 0, stream>>>(group_table, aggregate_count, string_extremes);
+      HYB_CUDA(cudaGetLastError());
+      ++out->launches;
+    }
+    // pack the occupied slots on the device; only they travel to the host
+    const uint64_t group_slots = table_control[0];
+    const size_t compact_words = std::max<uint64_t>(group_slots, 1) * per_slot_words;
+    const size_t compact_bytes = sizeof(uint64_t) * compact_words + sizeof(uint32_t) * std::max<uint64_t>(group_slots, 1) + 64;
+    void* compact = nullptr;
+    HYB_TRY(iteration.alloc(compact_bytes, &compact));
+    auto* compact_null_masks = reinterpret_cast<uint32_t*>(static_cast<unsigned long long*>(compact) + compact_words);
+    uint32_t* compact_cursor = compact_null_masks + std::max<uint64_t>(group_slots, 1);
+    HYB_CUDA(cudaMemsetAsync(compact_cursor, 0, sizeof(uint32_t), stream));
+    if (group_slots) {
+      aggregate_compact_kernel<<<slot_grid, 256, 0, stream>>>(group_table, aggregate_count, static_cast<uint32_t>(group_slots),
+                                                              static_cast<unsigned long long*>(compact), compact_null_masks,
+                                                              compact_cursor);
+      HYB_CUDA(cudaGetLastError());
+      ++out->launches;
+    }
+    std::vector<uint8_t> host(compact_bytes);
+    HYB_CUDA(cudaMemcpyAsync(host.data(), compact, compact_bytes, cudaMemcpyDeviceToHost, stream));
+    HYB_CUDA(cudaStreamSynchronize(stream));
+    parse_packed_groups(query, types, reinterpret_cast<const uint64_t*>(host.data()), group_slots, key_words, compact_words,
+                        &out->groups);
+    out->done = true;
   }
+  return HYB_OK;
+}
 
-  // ---- order the groups like the reference and materialise the result ---------------------------------------------
+// Orders the groups like the reference and builds the result: representative RowIDs, value and NULL columns.
+// `forced_immediate` >= 0: the partitioned exchange chose the order from all ranks' groups.
+static int materialise_aggregate_result(hyb_context* context, const Table* table, const hyb_aggregate_query* query,
+                                        const PosList* filter, bool exchanged, const AggregateTypes& types,
+                                        int forced_immediate, std::vector<HostGroup>& groups, uint32_t* launches,
+                                        std::unique_ptr<AggregateResult>* out_result) {
+  cudaStream_t stream = context->stream;
+  const uint32_t aggregate_count = query->aggregate_count;
   uint64_t input_rows = 0;
   for (const auto& group : groups) input_rows += group.rows;
   bool immediate = false;
@@ -2668,21 +2612,19 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
       // RowID is equivalent since no group-by column is written.
     }
     if (filter) {
-      void* d_positions = nullptr;
-      void* d_rows = nullptr;
-      HYB_TRY(device_alloc(context, sizeof(uint64_t) * positions.size(), &d_positions));
-      HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * positions.size(), &d_rows));
+      DeviceScratch scratch(context);
+      unsigned long long* d_positions = nullptr;
+      hyb_row_id* d_rows = nullptr;
+      HYB_TRY(scratch.alloc_array(positions.size(), &d_positions));
+      HYB_TRY(scratch.alloc_array(positions.size(), &d_rows));
       HYB_CUDA(cudaMemcpyAsync(d_positions, positions.data(), sizeof(uint64_t) * positions.size(), cudaMemcpyHostToDevice, stream));
       gather_row_ids_kernel<<<static_cast<uint32_t>((positions.size() + 255) / 256), 256, 0, stream>>>(
-          static_cast<const unsigned long long*>(d_positions), static_cast<uint32_t>(positions.size()), filter->d_row_ids,
-          static_cast<hyb_row_id*>(d_rows));
+          d_positions, static_cast<uint32_t>(positions.size()), filter->d_row_ids, d_rows);
       HYB_CUDA(cudaGetLastError());
       HYB_CUDA(cudaMemcpyAsync(result->row_ids.data(), d_rows, sizeof(hyb_row_id) * positions.size(), cudaMemcpyDeviceToHost, stream));
       HYB_CUDA(cudaStreamSynchronize(stream));
-      device_free(context, d_positions);
-      device_free(context, d_rows);
-      ++launches;
-    } else if (exchange) {
+      ++*launches;
+    } else if (exchanged) {
       for (size_t g = 0; g < groups.size(); ++g) result->row_ids[g] = immediate ? groups[g].row_max : groups[g].row_min;
     } else {
       for (size_t g = 0; g < groups.size(); ++g) result->row_ids[g] = position_to_row_id_host(table, positions[g]);
@@ -2691,12 +2633,13 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
   result->columns.resize(aggregate_count);
   for (uint32_t a = 0; a < aggregate_count; ++a) {
     const auto& def = query->aggregates[a];
+    const int32_t result_type = types.result_types[a];
     auto& column = result->columns[a];
-    column.value_type = result_types[a];
-    const size_t element = (result_types[a] == HYB_TYPE_INT32 || result_types[a] == HYB_TYPE_FLOAT32) ? 4 : 8;
+    column.value_type = result_type;
+    const size_t element = (result_type == HYB_TYPE_INT32 || result_type == HYB_TYPE_FLOAT32) ? 4 : 8;
     column.values.assign(group_count * element, 0);
     column.nulls.assign(group_count, 0);
-    const bool integral = input_types[a] == HYB_TYPE_INT32 || input_types[a] == HYB_TYPE_INT64;
+    const bool integral = types.input_types[a] == HYB_TYPE_INT32 || types.input_types[a] == HYB_TYPE_INT64;
     for (size_t g = 0; g < group_count; ++g) {
       const uint64_t count = synthesize_empty_row ? 0 : groups[g].counts[a];
       const uint64_t bits = synthesize_empty_row ? 0 : groups[g].accumulators[a];
@@ -2733,17 +2676,15 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
           break;
         }
         default: {  // MIN / MAX in the column type
-          if (result_types[a] == HYB_TYPE_STRING) {
-            std::memcpy(out, &bits, 8);  // the hyb_dictionary_position string_extreme_kernel wrote
-          } else if (result_types[a] == HYB_TYPE_INT32) {
+          if (result_type == HYB_TYPE_STRING || result_type == HYB_TYPE_INT64) {
+            std::memcpy(out, &bits, 8);  // strings: the hyb_dictionary_position string_extreme_kernel wrote
+          } else if (result_type == HYB_TYPE_INT32) {
             const int32_t value = static_cast<int32_t>(static_cast<int64_t>(bits));
             std::memcpy(out, &value, sizeof(value));
-          } else if (result_types[a] == HYB_TYPE_INT64) {
-            std::memcpy(out, &bits, 8);
           } else {
             double as_double;
             std::memcpy(&as_double, &bits, sizeof(as_double));
-            if (result_types[a] == HYB_TYPE_FLOAT32) {
+            if (result_type == HYB_TYPE_FLOAT32) {
               const float value = static_cast<float>(as_double);
               std::memcpy(out, &value, sizeof(value));
             } else {
@@ -2755,13 +2696,104 @@ static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query
       }
     }
   }
-  if (!kernel_timed) {
+  *out_result = std::move(result);
+  return HYB_OK;
+}
+
+// hyb_aggregate_hash with context->mutex held. `exchange` != nullptr: the groups of this rank are partial; they are
+// exchanged with the peer group's ranks and merged before the result is ordered and materialised. `tree` != nullptr: a
+// compiled expression tree (hyb_aggregate_hash_expression) every aggregated row must also satisfy.
+static int aggregate_hash_locked(hyb_context* context, const hyb_aggregate_query* query, hyb_aggregate_result_t* out_result,
+                                 const AggregateExchange* exchange, ExpressionTree* tree = nullptr) {
+  auto* table = find_table(context, query->table);
+  HYB_CHECK(table, HYB_ERR_NOT_FOUND, "unknown table handle");
+  PosList* filter = nullptr;
+  if (query->filter) {
+    filter = find_pos_list(context, query->filter);
+    HYB_CHECK(filter, HYB_ERR_NOT_FOUND, "unknown filter handle");
+    HYB_CHECK(filter->table == query->table, HYB_ERR_INVALID, "filter belongs to a different table");
+    HYB_CHECK(!filter->may_hold_null_rows, HYB_ERR_UNSUPPORTED,
+              "aggregating a PosList with NULL_ROW_IDs (an outer join's output) runs on the CPU operator");
+  }
+  HYB_TRY(sync_table_descriptors(context, table));
+
+  // ---- ANY: a group-by column the shim writes from the representative RowIDs (write_groupby_output, :421-537) -------
+  // It adds no accumulator: the other aggregates run exactly as without it (an all-ANY query is the group-by-only call,
+  // the reference's DISTINCT path), and its column of the result only names its type. It is checked before the others.
+  const uint32_t aggregate_count = query->aggregate_count;
+  std::vector<hyb_aggregate_def> kept;
+  std::vector<int32_t> any_types(aggregate_count, -1);
+  for (uint32_t a = 0; a < aggregate_count; ++a) {
+    const auto& def = query->aggregates[a];
+    if (def.function != HYB_AGG_ANY) {
+      kept.push_back(def);
+      continue;
+    }
+    HYB_CHECK(def.node_count == 1 && def.nodes[0].op == HYB_EXPR_COLUMN && def.nodes[0].column_id < table->column_count,
+              HYB_ERR_INVALID, "ANY takes a single column of the input table");
+    any_types[a] = table->column_types[def.nodes[0].column_id];
+  }
+  hyb_aggregate_query reduced = *query;
+  reduced.aggregate_count = static_cast<uint32_t>(kept.size());
+  reduced.aggregates = kept.data();
+  query = &reduced;  // the rest of the call never sees ANY
+
+  AggregateTypes types;
+  HYB_TRY(type_aggregates(context, table, query, &types));
+  timing_begin(context);
+  AggregateOutcome outcome;
+  uint64_t position_count = table->row_count();
+  uint64_t algorithmic_bytes = 0;
+  {
+    DeviceScratch predicate_scratch(context);  // the fused tests and the tree: no kernel reads them after the general path
+    FusedPredicates fused;
+    HYB_TRY(prepare_fused_predicates(context, table, query, tree, predicate_scratch, &fused));
+    outcome.launches = fused.launches;
+    if (filter) HYB_TRY(pos_list_total(context, filter, &position_count));
+    auto& slot = table->plan_memo[tree ? aggregate_signature(query) + "tree" + expression_tree_signature(*tree)
+                                       : aggregate_signature(query)];
+    if (!slot) slot = std::make_shared<AggregatePlanMemo>();
+    const auto memo = std::static_pointer_cast<AggregatePlanMemo>(slot);
+    algorithmic_bytes = aggregate_algorithmic_bytes(table, query, tree, types, filter, position_count, memo.get());
+    HYB_TRY(run_fast_path(context, table, query, fused, memo.get(), &outcome));
+    if (!outcome.done) HYB_TRY(run_general_path(context, table, query, filter, position_count, types, fused, &outcome));
+  }
+
+  int forced_immediate = -1;
+  if (exchange) {
+    HYB_CHECK(!filter, HYB_ERR_UNSUPPORTED, "distributed aggregation of position-filtered inputs is not on the GPU path");
+    // Low cardinality: one 32 KB block per rank, replicated result. A rank whose partial groups do not fit sends its block's
+    // header alone; every rank sees that in the same set of blocks and all of them switch to the partitioned exchange.
+    bool needs_partitioning = false;
+    HYB_TRY(exchange_partial_groups(context, *exchange, table, query, types.input_types, &outcome.groups, &needs_partitioning));
+    if (needs_partitioning) {
+      HYB_TRY(exchange_partial_groups_partitioned(context, *exchange, table, query, types.input_types, &outcome.groups,
+                                                  &forced_immediate));
+    }
+  }
+
+  std::unique_ptr<AggregateResult> result;
+  HYB_TRY(materialise_aggregate_result(context, table, query, filter, exchange != nullptr, types, forced_immediate,
+                                       outcome.groups, &outcome.launches, &result));
+  if (!outcome.kernel_timed) {
     timing_kernel_begin(context);
     timing_kernel_end(context);
   }
-  timing_end(context, launches, algorithmic_bytes, filter ? position_count : table->row_count(), group_count);
-  context->timing.stats.path = path;
+  timing_end(context, outcome.launches, algorithmic_bytes, filter ? position_count : table->row_count(), result->group_count);
+  context->timing.stats.path = outcome.path;
 
+  if (kept.size() < aggregate_count) {  // the ANY columns back in their slots
+    std::vector<AggregateColumn> columns(aggregate_count);
+    for (uint32_t a = 0, next = 0; a < aggregate_count; ++a) {
+      if (any_types[a] >= 0) {
+        columns[a].value_type = any_types[a];
+        columns[a].is_any = true;
+      } else {
+        columns[a] = std::move(result->columns[next++]);
+      }
+    }
+    result->columns = std::move(columns);
+  }
   const auto handle = context->next_handle++;
   context->aggregate_results.emplace(handle, std::move(result));
   *out_result = handle;
@@ -3177,6 +3209,17 @@ static int exchange_partial_groups_partitioned(hyb_context* context, const Aggre
   return HYB_OK;
 }
 
+// The argument checks every aggregate entry point makes before it takes the context's lock.
+static int check_aggregate_query(const hyb_aggregate_query* query) {
+  HYB_CHECK(query->groupby_count <= HYB_MAX_GROUPBY_COLUMNS, HYB_ERR_UNSUPPORTED, "too many group-by columns");
+  HYB_CHECK(query->aggregate_count <= HYB_MAX_AGGREGATES, HYB_ERR_UNSUPPORTED, "too many aggregates");
+  HYB_CHECK(query->predicate_count <= HYB_MAX_FUSED_PREDICATES, HYB_ERR_UNSUPPORTED, "too many fused predicates");
+  HYB_CHECK(query->groupby_count == 0 || query->groupby_column_ids, HYB_ERR_INVALID, "groupby_column_ids is NULL");
+  HYB_CHECK(query->aggregate_count == 0 || query->aggregates, HYB_ERR_INVALID, "aggregates is NULL");
+  HYB_CHECK(query->predicate_count == 0 || query->predicates, HYB_ERR_INVALID, "predicates is NULL");
+  return HYB_OK;
+}
+
 extern "C" {
 
 int hyb_aggregate_hash_expression(hyb_context* context, const hyb_aggregate_query* query,
@@ -3184,12 +3227,7 @@ int hyb_aggregate_hash_expression(hyb_context* context, const hyb_aggregate_quer
                                   hyb_aggregate_result_t* out_result) {
   HYB_CHECK(context && query && predicate && out_result, HYB_ERR_INVALID, "NULL argument");
   *out_result = 0;
-  HYB_CHECK(query->groupby_count <= HYB_MAX_GROUPBY_COLUMNS, HYB_ERR_UNSUPPORTED, "too many group-by columns");
-  HYB_CHECK(query->aggregate_count <= HYB_MAX_AGGREGATES, HYB_ERR_UNSUPPORTED, "too many aggregates");
-  HYB_CHECK(query->predicate_count <= HYB_MAX_FUSED_PREDICATES, HYB_ERR_UNSUPPORTED, "too many fused predicates");
-  HYB_CHECK(query->groupby_count == 0 || query->groupby_column_ids, HYB_ERR_INVALID, "groupby_column_ids is NULL");
-  HYB_CHECK(query->aggregate_count == 0 || query->aggregates, HYB_ERR_INVALID, "aggregates is NULL");
-  HYB_CHECK(query->predicate_count == 0 || query->predicates, HYB_ERR_INVALID, "predicates is NULL");
+  HYB_TRY(check_aggregate_query(query));
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
   const Table* table = find_table(context, query->table);
@@ -3202,12 +3240,7 @@ int hyb_aggregate_hash_expression(hyb_context* context, const hyb_aggregate_quer
 int hyb_aggregate_hash(hyb_context* context, const hyb_aggregate_query* query, hyb_aggregate_result_t* out_result) {
   HYB_CHECK(context && query && out_result, HYB_ERR_INVALID, "NULL argument");
   *out_result = 0;
-  HYB_CHECK(query->groupby_count <= HYB_MAX_GROUPBY_COLUMNS, HYB_ERR_UNSUPPORTED, "too many group-by columns");
-  HYB_CHECK(query->aggregate_count <= HYB_MAX_AGGREGATES, HYB_ERR_UNSUPPORTED, "too many aggregates");
-  HYB_CHECK(query->predicate_count <= HYB_MAX_FUSED_PREDICATES, HYB_ERR_UNSUPPORTED, "too many fused predicates");
-  HYB_CHECK(query->groupby_count == 0 || query->groupby_column_ids, HYB_ERR_INVALID, "groupby_column_ids is NULL");
-  HYB_CHECK(query->aggregate_count == 0 || query->aggregates, HYB_ERR_INVALID, "aggregates is NULL");
-  HYB_CHECK(query->predicate_count == 0 || query->predicates, HYB_ERR_INVALID, "predicates is NULL");
+  HYB_TRY(check_aggregate_query(query));
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
   return aggregate_hash_locked(context, query, out_result, nullptr);
@@ -3217,12 +3250,7 @@ int hyb_aggregate_hash_distributed(hyb_context* context, hyb_peer_group_t group_
                                    uint32_t chunk_id_base, uint64_t position_base, hyb_aggregate_result_t* out_result) {
   HYB_CHECK(context && query && out_result, HYB_ERR_INVALID, "NULL argument");
   *out_result = 0;
-  HYB_CHECK(query->groupby_count <= HYB_MAX_GROUPBY_COLUMNS, HYB_ERR_UNSUPPORTED, "too many group-by columns");
-  HYB_CHECK(query->aggregate_count <= HYB_MAX_AGGREGATES, HYB_ERR_UNSUPPORTED, "too many aggregates");
-  HYB_CHECK(query->predicate_count <= HYB_MAX_FUSED_PREDICATES, HYB_ERR_UNSUPPORTED, "too many fused predicates");
-  HYB_CHECK(query->groupby_count == 0 || query->groupby_column_ids, HYB_ERR_INVALID, "groupby_column_ids is NULL");
-  HYB_CHECK(query->aggregate_count == 0 || query->aggregates, HYB_ERR_INVALID, "aggregates is NULL");
-  HYB_CHECK(query->predicate_count == 0 || query->predicates, HYB_ERR_INVALID, "predicates is NULL");
+  HYB_TRY(check_aggregate_query(query));
   for (uint32_t a = 0; a < query->aggregate_count; ++a) {
     // Partial distinct sets and Welford states do not fit the exchanged partial groups. Every rank sees the same query,
     // so all ranks decline here, before any exchange.
@@ -3242,12 +3270,7 @@ int hyb_aggregate_hash_distributed(hyb_context* context, hyb_peer_group_t group_
       const auto& def = query->aggregates[a];
       if (def.function == HYB_AGG_COUNT_STAR) continue;  // no argument; its nodes are never read
       HYB_CHECK(def.node_count <= HYB_MAX_EXPR_NODES, HYB_ERR_INVALID, "bad expression length");
-      bool string_argument = false;
-      for (uint32_t n = 0; n < def.node_count; ++n) {
-        string_argument |= def.nodes[n].op == HYB_EXPR_COLUMN && def.nodes[n].column_id < table->column_count &&
-                           table->column_types[def.nodes[n].column_id] == HYB_TYPE_STRING;
-      }
-      HYB_CHECK(def.function != HYB_AGG_ANY && !string_argument, HYB_ERR_UNSUPPORTED,
+      HYB_CHECK(def.function != HYB_AGG_ANY && !has_string_argument(table, def), HYB_ERR_UNSUPPORTED,
                 "distributed ANY and aggregates over string columns run on the CPU operator");
     }
   }
