@@ -1619,10 +1619,16 @@ static int32_t calculate_radix_bits(uint64_t build_side_size) {
   return static_cast<int32_t>(std::min<size_t>(8, static_cast<size_t>(std::ceil(std::log2(cluster_count)))));
 }
 
+// Grid of a kernel that strides over `tiles` tiles: at most `blocks_per_sm` CTAs per SM, and at least one CTA.
+static uint32_t tile_grid(const hyb_context* context, uint32_t tiles, int blocks_per_sm) {
+  return std::max<uint32_t>(1, std::min<uint32_t>(tiles, context->sm_count * std::max(blocks_per_sm, 1)));
+}
+
 struct SideInfo {
   Table* table = nullptr;
   PosList* filter = nullptr;
   KeySource source{};
+  uint32_t column_id = 0;
   int32_t data_type = 0;
   uint64_t positions = 0;
 };
@@ -1631,6 +1637,7 @@ static int prepare_side(hyb_context* context, const hyb_join_side* side, SideInf
   out->table = find_table(context, side->table);
   HYB_CHECK(out->table, HYB_ERR_NOT_FOUND, "unknown table handle");
   HYB_CHECK(side->column_id < out->table->column_count, HYB_ERR_INVALID, "join column out of range");
+  out->column_id = side->column_id;
   out->data_type = out->table->chunk_count() ? out->table->column_types[side->column_id] : HYB_TYPE_INT32;
   HYB_CHECK(out->data_type == HYB_TYPE_INT32 || out->data_type == HYB_TYPE_INT64, HYB_ERR_UNSUPPORTED,
             "JoinHash on the device supports int32/int64 key columns; other key types run on the CPU operator");
@@ -1671,10 +1678,9 @@ static int prepare_side(hyb_context* context, const hyb_join_side* side, SideInf
 
 // Key bounds of the (whole) key column of a join side, cached on the table. A filtered side uses the same bounds: they
 // cover a superset of its keys.
-static int column_key_bounds(hyb_context* context, const SideInfo& side, uint32_t column_id, Table::KeyBounds* out,
-                             uint32_t* launches) {
+static int column_key_bounds(hyb_context* context, const SideInfo& side, Table::KeyBounds* out, uint32_t* launches) {
   Table* table = side.table;
-  const auto cached = table->key_bounds.find(column_id);
+  const auto cached = table->key_bounds.find(side.column_id);
   if (cached != table->key_bounds.end()) {
     *out = cached->second;
     return HYB_OK;
@@ -1685,18 +1691,17 @@ static int column_key_bounds(hyb_context* context, const SideInfo& side, uint32_
     whole.filter = nullptr;
     HYB_TRY(get_tile_map(context, table, kJoinTileRows, &whole.tile_map, &whole.tile_count));
     whole.position_count = table->row_count();
-    void* device_bounds = nullptr;
-    HYB_TRY(device_alloc(context, 6 * sizeof(long long), &device_bounds));
+    DeviceScratch scratch(context);
+    long long* device_bounds = nullptr;
+    HYB_TRY(scratch.alloc_array(6, &device_bounds));
     const long long initial[6] = {0x7FFFFFFFFFFFFFFFll, -0x7FFFFFFFFFFFFFFFll - 1, 0, -1ll, 0, 0};
     HYB_CUDA(cudaMemcpyAsync(device_bounds, initial, sizeof(initial), cudaMemcpyHostToDevice, context->stream));
-    const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>(whole.tile_count, context->sm_count * 8));
-    join_key_bounds_kernel<<<grid, kJoinThreads, 0, context->stream>>>(whole, static_cast<long long*>(device_bounds));
+    join_key_bounds_kernel<<<tile_grid(context, whole.tile_count, 8), kJoinThreads, 0, context->stream>>>(whole, device_bounds);
     HYB_CUDA(cudaGetLastError());
     ++*launches;
     long long host_bounds[6] = {};
     HYB_CUDA(cudaMemcpyAsync(host_bounds, device_bounds, sizeof(host_bounds), cudaMemcpyDeviceToHost, context->stream));
     HYB_CUDA(cudaStreamSynchronize(context->stream));
-    device_free(context, device_bounds);
     bounds.has_values = host_bounds[2] != 0;
     bounds.min = host_bounds[0];
     bounds.max = host_bounds[1];
@@ -1706,7 +1711,7 @@ static int column_key_bounds(hyb_context* context, const SideInfo& side, uint32_
       while (bounds.constant_low_bits < 16 && !((varying >> bounds.constant_low_bits) & 1ull)) ++bounds.constant_low_bits;
     }
   }
-  table->key_bounds.emplace(column_id, bounds);
+  table->key_bounds.emplace(side.column_id, bounds);
   *out = bounds;
   return HYB_OK;
 }
@@ -1718,25 +1723,391 @@ static int run_exclusive_scan(hyb_context* context, const uint32_t* in, unsigned
     if (total_out) HYB_CUDA(cudaMemsetAsync(total_out, 0, sizeof(unsigned long long), context->stream));
     return HYB_OK;
   }
-  void* status = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{tile_count} + 1), &status));
+  DeviceScratch scratch(context);  // the look-back status words; the next user of the block is queued after the scan
+  unsigned long long* status = nullptr;
+  HYB_TRY(scratch.alloc_array(size_t{tile_count} + 1, &status));
   HYB_CUDA(cudaMemsetAsync(status, 0, sizeof(uint64_t) * (size_t{tile_count} + 1), context->stream));
-  const uint32_t grid = std::min<uint32_t>(tile_count, context->sm_count * 4);
-  exclusive_scan_kernel<<<grid, kJoinThreads, 0, context->stream>>>(
-      in, out, count, static_cast<unsigned long long*>(status),
-      reinterpret_cast<uint32_t*>(static_cast<unsigned long long*>(status) + tile_count), total_out);
+  exclusive_scan_kernel<<<tile_grid(context, tile_count, 4), kJoinThreads, 0, context->stream>>>(
+      in, out, count, status, reinterpret_cast<uint32_t*>(status + tile_count), total_out);
   HYB_CUDA(cudaGetLastError());
-  device_free(context, status);
   return HYB_OK;
+}
+
+// The partition-count sequence of every probe pass and every partitioning: `count` launches the kernel that fills
+// params.histogram ([partition][tile] over `tiles` tiles), the exclusive scan turns it into params.run_starts and *total,
+// and join_partition_offsets_kernel writes the partition_count + 1 offsets. `write` runs between the scan and the offsets:
+// a probe's write kernel. A partitioning writes once it has read the offsets and passes nothing.
+template <typename Count, typename Write>
+static int count_partitions(hyb_context* context, const ProbeParams& params, uint32_t tiles, unsigned long long* total,
+                            unsigned long long* offsets, Count&& count, Write&& write) {
+  HYB_TRY(count());
+  // the kernels read run_starts through ProbeParams, hence const there; the scan is what fills it
+  HYB_TRY(run_exclusive_scan(context, params.histogram, const_cast<unsigned long long*>(params.run_starts),
+                             size_t{params.partition_count} * tiles, total));
+  HYB_TRY(write());
+  join_partition_offsets_kernel<<<(params.partition_count + 1 + 127) / 128, 128, 0, context->stream>>>(
+      params.run_starts, total, params.partition_count, tiles, offsets);
+  HYB_CUDA(cudaGetLastError());
+  return HYB_OK;
+}
+
+static int no_write() { return HYB_OK; }
+
+// ---- JoinHash stages (join_hash_locked) --------------------------------------------------------------------------------
+
+// The table over the build side. Dense key domain (range of the build column <= 8x its rows): direct-address table, one
+// uint32 per key value — or, when the build keys strictly increase with the build position, the 2-bits-per-key-value
+// rank table. Otherwise: bucketised open addressing at load factor <= 0.5.
+struct JoinTablePlan {
+  uint32_t kind = HYB_JOIN_PATH_TABLE_HASH;  // HYB_JOIN_PATH_TABLE_*
+  bool direct = false;                       // a direct-address table (shifted or not) or the rank table
+  bool rank = false;
+  bool wide = false;                         // int64 keys on either side
+  uint32_t direct_shift = 0;                 // the build keys agree in these low bits (one rank's share of an exchange)
+  unsigned long long key_span = 0, direct_span = 0;
+  uint64_t bucket_count = 1, slot_count = 0;
+  size_t slot_bytes = 0;
+};
+
+static int plan_join_table(const Table::KeyBounds& bounds, const SideInfo& build, const SideInfo& probe,
+                           const ContextOptions& options, JoinTablePlan* out) {
+  JoinTablePlan& plan = *out;
+  plan.wide = build.data_type == HYB_TYPE_INT64 || probe.data_type == HYB_TYPE_INT64;
+  plan.key_span = static_cast<unsigned long long>(bounds.max) - static_cast<unsigned long long>(bounds.min);
+  // options.join_table overrides the choice (the parity tests run every case with every table kind).
+  const bool force_hash = options.join_table == ContextOptions::kHash;
+  const bool force_direct = options.join_table == ContextOptions::kDirect;
+  plan.direct_shift = bounds.constant_low_bits;
+  plan.direct_span = plan.key_span >> plan.direct_shift;
+  plan.direct = bounds.has_values && build.positions > 0 && plan.direct_span < 0xFFFFFFE0ull && !force_hash &&
+                (plan.direct_span < 8 * build.positions + 65'536 ||
+                 (options.join_table != ContextOptions::kAuto && plan.direct_span < (1ull << 28)));
+  // Rank table: positions must grow with the keys — the column does (cached with the key bounds) and a PosList on top of
+  // it keeps the table order.
+  plan.rank = plan.direct && !force_direct && bounds.strictly_increasing && plan.key_span < 0xFFFFFFE0ull &&
+              (!build.filter || build.filter->ascending);
+  while (plan.bucket_count * 2 < build.positions) plan.bucket_count <<= 1;  // >= positions / 2 buckets -> load factor <= 0.5
+  HYB_CHECK(plan.bucket_count * 4 < 0xFFFFFFF0ull, HYB_ERR_UNSUPPORTED, "build side too large for 32-bit slot indexes");
+  plan.slot_count = plan.rank ? (plan.key_span >> 5) + 1 : plan.direct ? plan.direct_span + 1 : plan.bucket_count * 4;
+  plan.slot_bytes = plan.direct && !plan.rank ? sizeof(uint32_t) : sizeof(uint64_t);
+  plan.kind = plan.rank     ? HYB_JOIN_PATH_TABLE_RANK
+              : plan.direct ? (plan.direct_shift ? HYB_JOIN_PATH_TABLE_DIRECT_SHIFTED : HYB_JOIN_PATH_TABLE_DIRECT)
+              : plan.wide   ? HYB_JOIN_PATH_TABLE_HASH_WIDE
+                            : HYB_JOIN_PATH_TABLE_HASH;
+  return HYB_OK;
+}
+
+// Allocates the table's slots, the control words ([0] duplicate keys, [1] NULL build keys, [2] output overflow, [4..5] the
+// probe's total, u64) and an int64 hash table's keys, and queues the build kernels. Kernel time starts with them.
+static int build_join_table(hyb_context* context, DeviceScratch& scratch, const JoinTablePlan& plan,
+                            const Table::KeyBounds& bounds, const SideInfo& build, HashTable* out_table, uint32_t** out_control,
+                            uint32_t* launches) {
+  cudaStream_t stream = context->stream;
+  void* slots = nullptr;
+  uint32_t* control = nullptr;
+  long long* wide_keys = nullptr;
+  HYB_TRY(scratch.alloc(plan.slot_bytes * plan.slot_count, &slots));
+  HYB_CUDA(cudaMemsetAsync(slots, plan.rank ? 0x00 : 0xFF, plan.slot_bytes * plan.slot_count, stream));
+  HYB_TRY(scratch.alloc_array(16, &control));
+  HYB_CUDA(cudaMemsetAsync(control, 0, 64, stream));
+  if (plan.kind == HYB_JOIN_PATH_TABLE_HASH_WIDE) {
+    // every position a slot can name is written by join_wide_keys_kernel: no initialisation needed
+    HYB_TRY(scratch.alloc_array(std::max<uint64_t>(build.positions, 1), &wide_keys));
+  }
+  HashTable& table = *out_table;
+  table = HashTable{};
+  table.slots = static_cast<unsigned long long*>(slots);  // non-NULL also in direct / rank mode: "a table exists"
+  table.bucket_mask = static_cast<uint32_t>(plan.bucket_count - 1);
+  table.wide_keys = wide_keys;
+  if (plan.rank) {
+    table.rank_blocks = static_cast<uint2*>(slots);
+    table.direct_min = bounds.min;
+    table.direct_range = plan.key_span + 1;
+  } else if (plan.direct) {
+    table.direct = static_cast<uint32_t*>(slots);
+    table.direct_min = bounds.min;
+    table.direct_range = plan.direct_span + 1;
+    table.direct_shift = plan.direct_shift;
+  }
+  *out_control = control;
+  const uint32_t build_grid = tile_grid(context, build.source.tile_count, 8);
+  timing_kernel_begin(context);
+  if (build.source.tile_count) {
+    BuildParams params{};
+    params.source = build.source;
+    params.table = table;
+    params.wide_keys_out = wide_keys;
+    params.flags = control;
+    if (wide_keys) {
+      join_wide_keys_kernel<<<build_grid, kJoinThreads, 0, stream>>>(params);
+      HYB_CUDA(cudaGetLastError());
+      ++*launches;
+    }
+    if (plan.rank) {
+      join_build_rank_kernel<<<build_grid, kJoinThreads, 0, stream>>>(params);
+    } else {
+      join_build_kernel<<<build_grid, kJoinThreads, 0, stream>>>(params);
+    }
+    HYB_CUDA(cudaGetLastError());
+    ++*launches;
+  }
+  return HYB_OK;
+}
+
+// Which probe kernels run.
+struct ProbePlan {
+  bool span = false;       // the 8192-row span kernels (else the 4096-row tile kernels)
+  uint32_t tile_fast = 0;  // ProbeParams::fast of the tile kernels, whose lean path knows the direct table only
+};
+
+static ProbePlan plan_probe(const JoinTablePlan& table, const SideInfo& probe, int32_t mode, const ContextOptions& options) {
+  // Lean path of the case that dominates (Inner, dense unique build side): 1 = int32 keys on both sides, 2 = int64 probe
+  // keys against a (possibly shifted) direct table.
+  const uint32_t fast =
+      (mode == HYB_JOIN_INNER && table.direct)
+          ? ((table.direct_shift == 0 && !table.wide) ? 1u : ((!table.rank && probe.data_type == HYB_TYPE_INT64) ? 2u : 0u))
+          : 0u;
+  ProbePlan plan;
+  plan.tile_fast = table.rank ? 0u : fast;
+  // Span kernels: every probe segment must decode with a lean codec (plain values or FrameOfReference in a
+  // FixedWidthIntegerVector, no NULL vector); anything else keeps the tile kernels, which pick a decoder per tile.
+  plan.span = options.join_span && fast != 0 && !probe.filter && probe.source.tile_count > 0;
+  const Table* source = probe.table;
+  for (uint32_t chunk = 0; chunk < source->chunk_count() && plan.span; ++chunk) {
+    const DevSegment& segment = source->segments[size_t{chunk} * source->column_count + probe.column_id];
+    const bool plain64 = segment.encoding == HYB_ENC_UNENCODED && segment.data_type == HYB_TYPE_INT64;
+    plan.span = !segment.nulls && segment.encoding != HYB_ENC_DICTIONARY &&
+                !(segment.encoding == HYB_ENC_FRAME_OF_REFERENCE && segment.vector_type == HYB_VEC_BITPACKED) &&
+                (fast == 2) == plain64;
+  }
+  return plan;
+}
+
+// What every probe pass of one join shares.
+struct ProbeSetup {
+  ProbeParams params{};  // the tile kernels' parameters; each pass fills in its output blocks
+  void (*count_kernel)(const ProbeParams) = nullptr;
+  void (*write_kernel)(const ProbeParams) = nullptr;
+  uint32_t count_grid = 1, write_grid = 1;
+  KeySource span_source{};  // the span kernels: the probe side in kSpanRows-row spans
+  bool rank = false;        // span kernel variants
+  bool ballot = false;
+  unsigned long long* total = nullptr;  // output rows of the pass (device)
+};
+
+static int prepare_probe(hyb_context* context, DeviceScratch& scratch, const JoinTablePlan& plan, const ProbePlan& probe_plan,
+                         const SideInfo& build, const SideInfo& probe, int32_t mode, uint32_t partition_count,
+                         const HashTable& table, uint32_t* control, ProbeSetup* out) {
+  out->span_source = probe.source;
+  if (probe_plan.span) HYB_TRY(get_tile_map(context, probe.table, kSpanRows, &out->span_source.tile_map, &out->span_source.tile_count));
+  // Hash tables: the count kernel keeps match + partition per probe slot so that the write kernel does not repeat the
+  // random table accesses. Direct-address / rank tables are probed sequentially or from L2; looking up twice is cheaper
+  // than 10 bytes/row.
+  const bool store_matches = !plan.direct;
+  out->count_kernel = store_matches ? join_probe_count_kernel<true> : join_probe_count_kernel<false>;
+  out->write_kernel = store_matches ? join_probe_write_kernel<true> : join_probe_write_kernel<false>;
+  int count_blocks = 1, write_blocks = 1;
+  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&count_blocks, out->count_kernel, kJoinThreads, 0));
+  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&write_blocks, out->write_kernel, kJoinThreads, 0));
+  const uint32_t probe_tiles = probe.source.tile_count;
+  out->count_grid = tile_grid(context, probe_tiles, count_blocks);
+  out->write_grid = tile_grid(context, probe_tiles, write_blocks);
+  out->rank = plan.rank;
+  out->ballot = context->options.join_ballot_rank;
+  out->total = reinterpret_cast<unsigned long long*>(control + 4);
+  if (!probe_tiles) return HYB_OK;
+  ProbeParams& params = out->params;
+  const size_t probe_slots = size_t{probe_tiles} * kJoinTileRows;
+  if (store_matches) {
+    HYB_TRY(scratch.alloc_array(probe_slots, &params.matches));
+    HYB_TRY(scratch.alloc_array(probe_slots, &params.partitions));
+  }
+  // sized for the tile kernels as well: a duplicate build key sends a span-path call back to them
+  unsigned long long* run_starts = nullptr;
+  HYB_TRY(scratch.alloc_array(size_t{partition_count} * probe_tiles, &params.histogram));
+  HYB_TRY(scratch.alloc_array(size_t{partition_count} * probe_tiles, &run_starts));
+  params.probe = probe.source;
+  params.build = build.source;
+  params.table = table;
+  if (build.source.tile_count == 0) params.table.slots = nullptr;
+  params.mode = mode;
+  params.partition_mask = partition_count - 1;
+  params.partition_count = partition_count;
+  params.unique_build = 1;  // optimistic: a flag raised by the build kernel sends us to rerun_with_duplicates
+  params.fast = probe_plan.tile_fast;
+  params.build_is_empty = build.positions == 0;
+  params.flags = control;
+  params.run_starts = run_starts;
+  params.overflow = control + 2;
+  return HYB_OK;
+}
+
+// The result's output blocks for `capacity` rows (the previous pass's blocks go back to the cache): the result owns them.
+static int allocate_join_outputs(hyb_context* context, JoinResult* result, uint64_t capacity) {
+  device_free(context, result->d_probe);
+  device_free(context, result->d_build);
+  result->d_probe = nullptr;
+  result->d_build = nullptr;
+  void* out_probe = nullptr;
+  void* out_build = nullptr;
+  HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * std::max<uint64_t>(capacity, 1), &out_probe));
+  result->d_probe = static_cast<hyb_row_id*>(out_probe);
+  const int32_t mode = result->mode;
+  if (mode != HYB_JOIN_SEMI && mode != HYB_JOIN_ANTI_NULL_AS_TRUE && mode != HYB_JOIN_ANTI_NULL_AS_FALSE) {
+    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * std::max<uint64_t>(capacity, 1), &out_build));
+    result->d_build = static_cast<hyb_row_id*>(out_build);
+  }
+  result->capacity = capacity;
+  return HYB_OK;
+}
+
+// One probe pass: count -> scan -> output blocks of `capacity` rows -> write -> partition offsets, all queued without a
+// host round trip. `span`: the span kernels over setup.span_source; otherwise the tile kernels.
+static int run_probe_pass(hyb_context* context, DeviceScratch& scratch, ProbeSetup& setup, bool span, uint64_t capacity,
+                          JoinResult* result, uint32_t* launches) {
+  cudaStream_t stream = context->stream;
+  ProbeParams& params = setup.params;
+  ProbeParams span_params = params;
+  span_params.probe = setup.span_source;
+  const uint32_t tiles = span ? setup.span_source.tile_count : params.probe.tile_count;
+  const size_t counter_bytes = sizeof(uint32_t) * kSpanWarps * params.partition_count;
+  const size_t write_bytes = sizeof(uint2) * kSpanRows + counter_bytes;
+  const auto count_spans = setup.rank ? join_span_count_kernel<kTableRank> : join_span_count_kernel<kTableDirect>;
+  const auto write_spans =
+      setup.rank ? (setup.ballot ? join_span_write_kernel<kTableRank, true> : join_span_write_kernel<kTableRank, false>)
+                 : (setup.ballot ? join_span_write_kernel<kTableDirect, true> : join_span_write_kernel<kTableDirect, false>);
+  uint16_t* fine_counts = nullptr;
+  if (span) {
+    HYB_CUDA(cudaFuncSetAttribute(write_spans, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(write_bytes)));
+    HYB_TRY(scratch.alloc_array(size_t{tiles} * kSpanWarps * params.partition_count, &fine_counts));
+  }
+  const auto count = [&]() -> int {
+    if (span) {
+      count_spans<<<tiles, kSpanThreads, counter_bytes, stream>>>(span_params, fine_counts);
+    } else {
+      setup.count_kernel<<<setup.count_grid, kJoinThreads, 0, stream>>>(params);
+    }
+    HYB_CUDA(cudaGetLastError());
+    return HYB_OK;
+  };
+  const auto write = [&]() -> int {
+    HYB_TRY(allocate_join_outputs(context, result, capacity));
+    params.out_probe = span_params.out_probe = result->d_probe;
+    params.out_build = span_params.out_build = result->d_build;
+    params.out_capacity = span_params.out_capacity = capacity;
+    if (span) {
+      write_spans<<<tiles, kSpanThreads, write_bytes, stream>>>(span_params, fine_counts);
+    } else {
+      setup.write_kernel<<<setup.write_grid, kJoinThreads, 0, stream>>>(params);
+    }
+    HYB_CUDA(cudaGetLastError());
+    return HYB_OK;
+  };
+  HYB_TRY(count_partitions(context, params, tiles, setup.total,
+                           reinterpret_cast<unsigned long long*>(result->d_partition_offsets), count, write));
+  *launches += 4;
+  return HYB_OK;
+}
+
+// Duplicate build keys: build the position lists (PosHashTable::finalize, join_hash_steps.hpp:147-175), size the output
+// exactly (count + scan, read the total) and probe again with the tile kernels: the span kernels are for unique build sides.
+static int rerun_with_duplicates(hyb_context* context, DeviceScratch& scratch, const JoinTablePlan& plan, const SideInfo& build,
+                                 const HashTable& table, ProbeSetup& setup, JoinResult* result, uint32_t* launches) {
+  cudaStream_t stream = context->stream;
+  const uint64_t slot_count = plan.slot_count;
+  const uint32_t build_grid = tile_grid(context, build.source.tile_count, 8);
+  uint32_t* dup_counts = nullptr;  // counts | cursors
+  unsigned long long* dup_offsets = nullptr;
+  uint32_t* dup_positions = nullptr;
+  HYB_TRY(scratch.alloc_array(slot_count * 2, &dup_counts));
+  HYB_CUDA(cudaMemsetAsync(dup_counts, 0, sizeof(uint32_t) * slot_count * 2, stream));
+  HYB_TRY(scratch.alloc_array(slot_count, &dup_offsets));
+  HYB_TRY(scratch.alloc_array(std::max<uint64_t>(build.positions, 1), &dup_positions));
+  timing_kernel_begin(context);
+  join_count_duplicates_kernel<<<build_grid, kJoinThreads, 0, stream>>>(build.source, table, dup_counts);
+  HYB_CUDA(cudaGetLastError());
+  HYB_TRY(run_exclusive_scan(context, dup_counts, dup_offsets, slot_count, nullptr));
+  join_fill_positions_kernel<<<build_grid, kJoinThreads, 0, stream>>>(build.source, table, dup_offsets, dup_counts + slot_count,
+                                                                      dup_positions);
+  HYB_CUDA(cudaGetLastError());
+  join_sort_positions_kernel<<<static_cast<uint32_t>((slot_count + 255) / 256), 256, 0, stream>>>(
+      dup_counts, dup_offsets, static_cast<uint32_t>(slot_count), dup_positions);
+  HYB_CUDA(cudaGetLastError());
+  *launches += 4;
+  ProbeParams& params = setup.params;
+  params.unique_build = 0;
+  params.dup_counts = dup_counts;
+  params.dup_offsets = dup_offsets;
+  params.dup_positions = dup_positions;
+  setup.count_kernel<<<setup.count_grid, kJoinThreads, 0, stream>>>(params);
+  HYB_CUDA(cudaGetLastError());
+  HYB_TRY(run_exclusive_scan(context, params.histogram, const_cast<unsigned long long*>(params.run_starts),
+                             size_t{params.partition_count} * params.probe.tile_count, setup.total));
+  *launches += 2;
+  uint64_t total = 0;
+  HYB_CUDA(cudaMemcpyAsync(&total, setup.total, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
+  HYB_CUDA(cudaStreamSynchronize(stream));
+  HYB_CUDA(cudaMemsetAsync(params.overflow, 0, sizeof(uint32_t), stream));
+  HYB_TRY(run_probe_pass(context, scratch, setup, false, total, result, launches));
+  timing_kernel_end(context);
+  HYB_CUDA(cudaStreamSynchronize(stream));
+  return HYB_OK;
+}
+
+// Compulsory traffic of one side's keys (SURVEY.md §8d): the key column once, or a PosList's RowIDs and keys.
+static uint64_t join_key_bytes(const SideInfo& side) {
+  if (side.filter) return side.positions * (sizeof(hyb_row_id) + data_type_size(side.data_type));
+  uint64_t bytes = 0;
+  for (uint32_t chunk = 0; chunk < side.table->chunk_count(); ++chunk) {
+    const auto& segment = side.table->segments[size_t{chunk} * side.table->column_count + side.column_id];
+    bytes += segment.encoding == HYB_ENC_UNENCODED ? data_type_size(segment.data_type) * segment.row_count
+                                                   : vector_bytes(segment.vector_type, segment.bit_width, segment.row_count);
+    if (segment.encoding == HYB_ENC_FRAME_OF_REFERENCE) {
+      bytes += sizeof(int32_t) * ((segment.row_count + HYB_FOR_BLOCK_SIZE - 1) / HYB_FOR_BLOCK_SIZE);
+    }
+  }
+  return bytes;
+}
+
+// The hyb_join_path code of a join: its table kind, the probe kernels (when there were probe rows) and the rerun.
+static uint32_t join_path_code(const JoinTablePlan& table, const ProbePlan& probe, bool probed, bool rerun) {
+  uint32_t path = table.kind;
+  if (probed) path |= probe.span ? HYB_JOIN_PATH_PROBE_SPAN : probe.tile_fast ? HYB_JOIN_PATH_PROBE_TILE_LEAN : HYB_JOIN_PATH_PROBE_TILE;
+  if (rerun) path |= HYB_JOIN_PATH_RERUN;
+  return path;
+}
+
+// The count kernel of a kModePartition split: the probe's count kernel without a table or stored matches.
+static int launch_partition_count(hyb_context* context, const ProbeParams& params) {
+  int blocks = 1;
+  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, join_probe_count_kernel<false>, kJoinThreads, 0));
+  join_probe_count_kernel<false><<<tile_grid(context, params.probe.tile_count, blocks), kJoinThreads, 0, context->stream>>>(params);
+  HYB_CUDA(cudaGetLastError());
+  return HYB_OK;
+}
+
+// ProbeParams of the stable split of a side's {key, RowID} tuples by key & (partition_count - 1) (kModePartition): the
+// probe machinery without a table. `control`: 16 zeroed words, the scan's total at [4..5].
+static ProbeParams partition_params(const SideInfo& side, uint32_t partition_count, uint32_t chunk_id_base, uint32_t* control,
+                                    uint32_t* histogram, const unsigned long long* run_starts) {
+  ProbeParams params{};
+  params.probe = side.source;
+  params.build = side.source;
+  params.mode = kModePartition;
+  params.partition_mask = partition_count - 1;
+  params.partition_count = partition_count;
+  params.unique_build = 1;
+  params.flags = control;
+  params.histogram = histogram;
+  params.run_starts = run_starts;
+  params.overflow = control + 2;
+  params.chunk_id_base = chunk_id_base;
+  return params;
 }
 
 }  // namespace hyb
 
 using namespace hyb;
-
-extern "C" {
-
-}  // extern "C"
 
 // hyb_join_hash with context->mutex held (hyb_join_hash_distributed joins the received tuples through it).
 static int join_hash_locked(hyb_context* context, const hyb_join_side* build_side, const hyb_join_side* probe_side, int32_t mode,
@@ -1752,90 +2123,21 @@ static int join_hash_locked(hyb_context* context, const hyb_join_side* build_sid
   if (radix_bits < 0) radix_bits = calculate_radix_bits(build.positions);
   HYB_CHECK(radix_bits <= 8, HYB_ERR_INVALID, "radix_bits must be <= 8 (join_hash.cpp:113)");
   const uint32_t partition_count = 1u << radix_bits;
-  const bool wide = build.data_type == HYB_TYPE_INT64 || probe.data_type == HYB_TYPE_INT64;
   const bool semi_or_anti = mode == HYB_JOIN_SEMI || mode == HYB_JOIN_ANTI_NULL_AS_TRUE || mode == HYB_JOIN_ANTI_NULL_AS_FALSE;
   cudaStream_t stream = context->stream;
-  const ContextOptions options = context->options;
   uint32_t launches = 0;
   DeviceScratch scratch(context);  // every scratch block of this call goes back to the cache on every exit path
-
   timing_begin(context);
 
-  // ---- build -----------------------------------------------------------------------------------------------------
-  // Dense key domain (range of the build column <= 8x its rows): direct-address table, one uint32 per key value — or,
-  // when the build keys strictly increase with the build position, the 2-bits-per-key-value rank table.
-  // Otherwise: bucketised open addressing at load factor <= 0.5.
   Table::KeyBounds bounds{};
-  HYB_TRY(column_key_bounds(context, build, build_side->column_id, &bounds, &launches));
-  const unsigned long long key_span = static_cast<unsigned long long>(bounds.max) - static_cast<unsigned long long>(bounds.min);
-  // options.join_table overrides the choice (the parity tests run every case with every table kind).
-  const bool force_hash = options.join_table == ContextOptions::kHash;
-  const bool force_direct = options.join_table == ContextOptions::kDirect;
-  const uint32_t direct_shift = bounds.constant_low_bits;  // keys agree in these low bits (one rank's share of an exchange)
-  const unsigned long long direct_span = key_span >> direct_shift;
-  const bool direct = bounds.has_values && build.positions > 0 && direct_span < 0xFFFFFFE0ull && !force_hash &&
-                      (direct_span < 8 * build.positions + 65'536 ||
-                       (options.join_table != ContextOptions::kAuto && direct_span < (1ull << 28)));
-  // Rank table: positions must grow with the keys — the column does (cached with the key bounds) and a PosList on top of
-  // it keeps the table order.
-  const bool rank = direct && !force_direct && bounds.strictly_increasing && key_span < 0xFFFFFFE0ull &&
-                    (!build.filter || build.filter->ascending);
-  uint64_t bucket_count = 1;
-  while (bucket_count * 2 < build.positions) bucket_count <<= 1;  // >= positions / 2 buckets -> load factor <= 0.5
-  HYB_CHECK(bucket_count * 4 < 0xFFFFFFF0ull, HYB_ERR_UNSUPPORTED, "build side too large for 32-bit slot indexes");
-  const uint64_t slot_count = rank ? (key_span >> 5) + 1 : direct ? direct_span + 1 : bucket_count * 4;
-  const size_t slot_bytes = direct && !rank ? sizeof(uint32_t) : sizeof(uint64_t);
-  void* slots = nullptr;
-  void* wide_keys = nullptr;
-  void* control = nullptr;  // [0] duplicate keys, [1] NULL build keys, [2] output overflow, [4..5] total (u64)
-  HYB_TRY(scratch.alloc(slot_bytes * slot_count, &slots));
-  HYB_CUDA(cudaMemsetAsync(slots, rank ? 0x00 : 0xFF, slot_bytes * slot_count, stream));
-  HYB_TRY(scratch.alloc(64, &control));
-  HYB_CUDA(cudaMemsetAsync(control, 0, 64, stream));
-  auto* flags = static_cast<uint32_t*>(control);
-  auto* total_slot = reinterpret_cast<unsigned long long*>(flags + 4);
-  if (wide && !direct) {
-    // every position a slot can name is written by join_wide_keys_kernel: no initialisation needed
-    HYB_TRY(scratch.alloc(sizeof(long long) * std::max<uint64_t>(build.positions, 1), &wide_keys));
-  }
+  HYB_TRY(column_key_bounds(context, build, &bounds, &launches));
+  JoinTablePlan table_plan;
+  HYB_TRY(plan_join_table(bounds, build, probe, context->options, &table_plan));
   HashTable table{};
-  table.slots = static_cast<unsigned long long*>(slots);  // non-NULL also in direct / rank mode: "a table exists"
-  table.bucket_mask = static_cast<uint32_t>(bucket_count - 1);
-  table.wide_keys = static_cast<const long long*>(wide_keys);
-  if (rank) {
-    table.rank_blocks = static_cast<uint2*>(slots);
-    table.direct_min = bounds.min;
-    table.direct_range = key_span + 1;
-  } else if (direct) {
-    table.direct = static_cast<uint32_t*>(slots);
-    table.direct_min = bounds.min;
-    table.direct_range = direct_span + 1;
-    table.direct_shift = direct_shift;
-  }
-  const uint32_t build_grid = std::max<uint32_t>(1, std::min<uint32_t>(build.source.tile_count, context->sm_count * 8));
-  timing_kernel_begin(context);
-  if (build.source.tile_count) {
-    BuildParams build_params{};
-    build_params.source = build.source;
-    build_params.table = table;
-    build_params.wide_keys_out = static_cast<long long*>(wide_keys);
-    build_params.flags = flags;
-    if (wide_keys) {
-      join_wide_keys_kernel<<<build_grid, kJoinThreads, 0, stream>>>(build_params);
-      HYB_CUDA(cudaGetLastError());
-      ++launches;
-    }
-    if (rank) {
-      join_build_rank_kernel<<<build_grid, kJoinThreads, 0, stream>>>(build_params);
-    } else {
-      join_build_kernel<<<build_grid, kJoinThreads, 0, stream>>>(build_params);
-    }
-    HYB_CUDA(cudaGetLastError());
-    ++launches;
-  }
+  uint32_t* control = nullptr;
+  HYB_TRY(build_join_table(context, scratch, table_plan, bounds, build, &table, &control, &launches));
 
-  // ---- probe -----------------------------------------------------------------------------------------------------
-  auto result = std::make_unique<JoinResult>();
+  auto result = std::make_unique<JoinResult>();  // owns its output blocks and partition offsets
   result->mode = mode;
   result->build_table = build_side->table;
   result->probe_table = probe_side->table;
@@ -1848,228 +2150,28 @@ static int join_hash_locked(hyb_context* context, const hyb_join_side* build_sid
   result->d_partition_offsets = static_cast<uint64_t*>(partition_offsets);
   HYB_CUDA(cudaMemsetAsync(partition_offsets, 0, sizeof(uint64_t) * (size_t{partition_count} + 2), stream));
 
-  const uint32_t probe_tiles = probe.source.tile_count;
-  // Lean path of the case that dominates (Inner, dense unique build side): 1 = int32 keys on both sides, 2 = int64 probe
-  // keys against a (possibly shifted) direct table.
-  const uint32_t fast = (mode == HYB_JOIN_INNER && (direct || rank))
-                            ? ((direct_shift == 0 && !wide) ? 1u : ((!rank && probe.data_type == HYB_TYPE_INT64) ? 2u : 0u))
-                            : 0u;
-  // Span kernels: every probe segment must decode with a lean codec (plain values or FrameOfReference in a
-  // FixedWidthIntegerVector, no NULL vector); anything else keeps the tile kernels, which pick a decoder per tile.
-  bool use_span = options.join_span && fast != 0 && !probe.filter && probe_tiles > 0;
-  if (use_span) {
-    const Table* table_ptr = probe.table;
-    for (uint32_t chunk = 0; chunk < table_ptr->chunk_count() && use_span; ++chunk) {
-      const DevSegment& segment = table_ptr->segments[size_t{chunk} * table_ptr->column_count + probe_side->column_id];
-      if (segment.nulls) use_span = false;
-      if (segment.encoding == HYB_ENC_DICTIONARY) use_span = false;
-      if (segment.encoding == HYB_ENC_FRAME_OF_REFERENCE && segment.vector_type == HYB_VEC_BITPACKED) use_span = false;
-      const bool plain64 = segment.encoding == HYB_ENC_UNENCODED && segment.data_type == HYB_TYPE_INT64;
-      if ((fast == 2) != plain64) use_span = false;
-    }
-  }
-  KeySource span_source = probe.source;
-  if (use_span) HYB_TRY(get_tile_map(context, probe.table, kSpanRows, &span_source.tile_map, &span_source.tile_count));
-  const uint32_t histogram_tiles = use_span ? span_source.tile_count : probe_tiles;
-
-  // Hash tables: the count kernel keeps match + partition per probe slot so that the write kernel does not repeat the
-  // random table accesses. Direct-address / rank tables are probed sequentially or from L2; looking up twice is cheaper
-  // than 10 bytes/row.
-  const bool store_matches = !direct;
-  const auto count_kernel = store_matches ? join_probe_count_kernel<true> : join_probe_count_kernel<false>;
-  const auto write_kernel = store_matches ? join_probe_write_kernel<true> : join_probe_write_kernel<false>;
-  int count_blocks = 1, write_blocks = 1;
-  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&count_blocks, count_kernel, kJoinThreads, 0));
-  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&write_blocks, write_kernel, kJoinThreads, 0));
-  const uint32_t count_grid = std::max<uint32_t>(1, std::min<uint32_t>(probe_tiles, context->sm_count * std::max(count_blocks, 1)));
-  const uint32_t write_grid = std::max<uint32_t>(1, std::min<uint32_t>(probe_tiles, context->sm_count * std::max(write_blocks, 1)));
-  const size_t probe_slots = size_t{probe_tiles} * kJoinTileRows;
-  void* matches = nullptr;
-  void* partitions = nullptr;
-  void* histogram = nullptr;
-  void* run_starts = nullptr;
-  void* dup_counts = nullptr;
-  void* dup_offsets = nullptr;
-  void* dup_positions = nullptr;
-  size_t histogram_entries = size_t{partition_count} * histogram_tiles;
-  ProbeParams params{};
-  uint32_t host_control[8] = {};
-  if (probe_tiles) {
-    if (store_matches) {
-      HYB_TRY(scratch.alloc(sizeof(uint32_t) * probe_slots, &matches));
-      HYB_TRY(scratch.alloc(probe_slots, &partitions));
-    }
-    // sized for the tile kernels as well: a duplicate build key sends a span-path call back to them
-    HYB_TRY(scratch.alloc(sizeof(uint32_t) * size_t{partition_count} * probe_tiles, &histogram));
-    HYB_TRY(scratch.alloc(sizeof(uint64_t) * size_t{partition_count} * probe_tiles, &run_starts));
-    params.probe = probe.source;
-    params.build = build.source;
-    params.table = table;
-    if (build.source.tile_count == 0) params.table.slots = nullptr;
-    params.mode = mode;
-    params.partition_mask = partition_count - 1;
-    params.partition_count = partition_count;
-    params.unique_build = 1;  // optimistic: a flag raised by the build kernel sends us to the position-list path below
-    params.fast = rank ? 0u : fast;  // the tile kernels' lean path knows the direct table only
-    params.build_is_empty = build.positions == 0;
-    params.flags = flags;
-    params.matches = static_cast<uint32_t*>(matches);
-    params.partitions = static_cast<uint8_t*>(partitions);
-    params.histogram = static_cast<uint32_t*>(histogram);
-    params.run_starts = static_cast<const unsigned long long*>(run_starts);
-    params.overflow = flags + 2;
-  }
-
-  const auto allocate_outputs = [&](uint64_t capacity) -> int {
-    device_free(context, result->d_probe);
-    device_free(context, result->d_build);
-    result->d_probe = nullptr;
-    result->d_build = nullptr;
-    void* out_probe = nullptr;
-    void* out_build = nullptr;
-    HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * std::max<uint64_t>(capacity, 1), &out_probe));
-    result->d_probe = static_cast<hyb_row_id*>(out_probe);
-    if (!semi_or_anti) {
-      HYB_TRY(device_alloc(context, sizeof(hyb_row_id) * std::max<uint64_t>(capacity, 1), &out_build));
-      result->d_build = static_cast<hyb_row_id*>(out_build);
-    }
-    result->capacity = capacity;
-    params.out_probe = result->d_probe;
-    params.out_build = result->d_build;
-    params.out_capacity = capacity;
-    return HYB_OK;
-  };
-
-  const auto run_probe = [&](uint64_t capacity) -> int {
-    // count -> scan -> write, all queued without a host round trip; `capacity` output rows are pre-allocated
-    count_kernel<<<count_grid, kJoinThreads, 0, stream>>>(params);
-    HYB_CUDA(cudaGetLastError());
-    HYB_TRY(run_exclusive_scan(context, static_cast<uint32_t*>(histogram), static_cast<unsigned long long*>(run_starts),
-                               histogram_entries, total_slot));
-    HYB_TRY(allocate_outputs(capacity));
-    write_kernel<<<write_grid, kJoinThreads, 0, stream>>>(params);
-    HYB_CUDA(cudaGetLastError());
-    join_partition_offsets_kernel<<<(partition_count + 1 + 127) / 128, 128, 0, stream>>>(
-        static_cast<const unsigned long long*>(run_starts), total_slot, partition_count, probe_tiles,
-        reinterpret_cast<unsigned long long*>(result->d_partition_offsets));
-    HYB_CUDA(cudaGetLastError());
-    launches += 4;
-    return HYB_OK;
-  };
-
-  const auto run_probe_spans = [&]() -> int {
-    ProbeParams span_params = params;
-    span_params.probe = span_source;
-    const uint32_t spans = span_source.tile_count;
-    const size_t counter_bytes = sizeof(uint32_t) * kSpanWarps * partition_count;
-    const size_t write_bytes = sizeof(uint2) * kSpanRows + counter_bytes;
-    const auto count_spans = rank ? join_span_count_kernel<kTableRank> : join_span_count_kernel<kTableDirect>;
-    const auto write_spans =
-        rank ? (options.join_ballot_rank ? join_span_write_kernel<kTableRank, true> : join_span_write_kernel<kTableRank, false>)
-             : (options.join_ballot_rank ? join_span_write_kernel<kTableDirect, true> : join_span_write_kernel<kTableDirect, false>);
-    HYB_CUDA(cudaFuncSetAttribute(write_spans, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(write_bytes)));
-    uint16_t* fine_counts = nullptr;
-    HYB_TRY(scratch.alloc_array(size_t{spans} * kSpanWarps * partition_count, &fine_counts));
-    count_spans<<<spans, kSpanThreads, counter_bytes, stream>>>(span_params, fine_counts);
-    HYB_CUDA(cudaGetLastError());
-    HYB_TRY(run_exclusive_scan(context, static_cast<uint32_t*>(histogram), static_cast<unsigned long long*>(run_starts),
-                               histogram_entries, total_slot));
-    HYB_TRY(allocate_outputs(probe.positions));
-    span_params.out_probe = params.out_probe;
-    span_params.out_build = params.out_build;
-    span_params.out_capacity = params.out_capacity;
-    write_spans<<<spans, kSpanThreads, write_bytes, stream>>>(span_params, fine_counts);
-    HYB_CUDA(cudaGetLastError());
-    join_partition_offsets_kernel<<<(partition_count + 1 + 127) / 128, 128, 0, stream>>>(
-        static_cast<const unsigned long long*>(run_starts), total_slot, partition_count, spans,
-        reinterpret_cast<unsigned long long*>(result->d_partition_offsets));
-    HYB_CUDA(cudaGetLastError());
-    launches += 4;
-    return HYB_OK;
-  };
-
-  if (probe_tiles) {
-    // With a unique build side every probe row emits at most one output row: probe.positions rows always suffice.
-    if (use_span) {
-      HYB_TRY(run_probe_spans());
-    } else {
-      HYB_TRY(run_probe(probe.positions));
-    }
-  }
+  const ProbePlan probe_plan = plan_probe(table_plan, probe, mode, context->options);
+  ProbeSetup setup;
+  HYB_TRY(prepare_probe(context, scratch, table_plan, probe_plan, build, probe, mode, partition_count, table, control, &setup));
+  const bool probed = probe.source.tile_count != 0;
+  // With a unique build side every probe row emits at most one output row: probe.positions rows always suffice.
+  if (probed) HYB_TRY(run_probe_pass(context, scratch, setup, probe_plan.span, probe.positions, result.get(), &launches));
   timing_kernel_end(context);
+  uint32_t host_control[8] = {};
   HYB_CUDA(cudaMemcpyAsync(host_control, control, sizeof(host_control), cudaMemcpyDeviceToHost, stream));
   HYB_CUDA(cudaStreamSynchronize(stream));  // the only host round trip of the operator (unique build side)
-  const bool has_duplicates = host_control[0] != 0;
+  const bool rerun = host_control[0] != 0 && !semi_or_anti && probed;
+  if (rerun) HYB_TRY(rerun_with_duplicates(context, scratch, table_plan, build, table, setup, result.get(), &launches));
 
-  if (has_duplicates && !semi_or_anti && probe_tiles) {
-    // Duplicate build keys: build the position lists (PosHashTable::finalize, join_hash_steps.hpp:147-175) and probe again
-    // (with the tile kernels: the span path is for unique build sides).
-    histogram_entries = size_t{partition_count} * probe_tiles;
-    HYB_TRY(scratch.alloc(sizeof(uint32_t) * slot_count * 2, &dup_counts));  // counts | cursors
-    HYB_CUDA(cudaMemsetAsync(dup_counts, 0, sizeof(uint32_t) * slot_count * 2, stream));
-    HYB_TRY(scratch.alloc(sizeof(uint64_t) * slot_count, &dup_offsets));
-    HYB_TRY(scratch.alloc(sizeof(uint32_t) * std::max<uint64_t>(build.positions, 1), &dup_positions));
-    timing_kernel_begin(context);
-    join_count_duplicates_kernel<<<build_grid, kJoinThreads, 0, stream>>>(build.source, table, static_cast<uint32_t*>(dup_counts));
-    HYB_CUDA(cudaGetLastError());
-    HYB_TRY(run_exclusive_scan(context, static_cast<uint32_t*>(dup_counts), static_cast<unsigned long long*>(dup_offsets),
-                               slot_count, nullptr));
-    join_fill_positions_kernel<<<build_grid, kJoinThreads, 0, stream>>>(
-        build.source, table, static_cast<unsigned long long*>(dup_offsets), static_cast<uint32_t*>(dup_counts) + slot_count,
-        static_cast<uint32_t*>(dup_positions));
-    HYB_CUDA(cudaGetLastError());
-    join_sort_positions_kernel<<<static_cast<uint32_t>((slot_count + 255) / 256), 256, 0, stream>>>(
-        static_cast<uint32_t*>(dup_counts), static_cast<unsigned long long*>(dup_offsets), static_cast<uint32_t>(slot_count),
-        static_cast<uint32_t*>(dup_positions));
-    HYB_CUDA(cudaGetLastError());
-    launches += 4;
-    params.unique_build = 0;
-    params.dup_counts = static_cast<const uint32_t*>(dup_counts);
-    params.dup_offsets = static_cast<const unsigned long long*>(dup_offsets);
-    params.dup_positions = static_cast<const uint32_t*>(dup_positions);
-    // size the output exactly: count + scan, read the total, then write
-    count_kernel<<<count_grid, kJoinThreads, 0, stream>>>(params);
-    HYB_CUDA(cudaGetLastError());
-    HYB_TRY(run_exclusive_scan(context, static_cast<uint32_t*>(histogram), static_cast<unsigned long long*>(run_starts),
-                               histogram_entries, total_slot));
-    uint64_t total = 0;
-    HYB_CUDA(cudaMemcpyAsync(&total, total_slot, sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
-    HYB_CUDA(cudaStreamSynchronize(stream));
-    HYB_CUDA(cudaMemsetAsync(flags + 2, 0, sizeof(uint32_t), stream));
-    HYB_TRY(run_probe(total));
-    timing_kernel_end(context);
-    HYB_CUDA(cudaStreamSynchronize(stream));
-  }
-
-  // Compulsory traffic (SURVEY.md §8d): each key once + each output RowID once.
-  const auto key_bytes = [](const SideInfo& side) -> uint64_t {
-    if (side.filter) return side.positions * (sizeof(hyb_row_id) + data_type_size(side.data_type));
-    uint64_t bytes = 0;
-    const uint32_t column = static_cast<uint32_t>((side.source.segments - side.table->d_segments) / std::max<uint32_t>(side.table->chunk_count(), 1));
-    for (uint32_t chunk = 0; chunk < side.table->chunk_count(); ++chunk) {
-      const auto& segment = side.table->segments[size_t{chunk} * side.table->column_count + column];
-      bytes += segment.encoding == HYB_ENC_UNENCODED ? data_type_size(segment.data_type) * segment.row_count
-                                                     : vector_bytes(segment.vector_type, segment.bit_width, segment.row_count);
-      if (segment.encoding == HYB_ENC_FRAME_OF_REFERENCE) {
-        bytes += sizeof(int32_t) * ((segment.row_count + HYB_FOR_BLOCK_SIZE - 1) / HYB_FOR_BLOCK_SIZE);
-      }
-    }
-    return bytes;
-  };
-  timing_end(context, launches, key_bytes(build) + key_bytes(probe), probe.positions, 0);
+  timing_end(context, launches, join_key_bytes(build) + join_key_bytes(probe), probe.positions, 0);
   timing_output_count(context, result->d_partition_offsets + partition_count, semi_or_anti ? 8 : 16);
-  uint32_t path = rank ? HYB_JOIN_PATH_TABLE_RANK
-                  : direct ? (direct_shift ? HYB_JOIN_PATH_TABLE_DIRECT_SHIFTED : HYB_JOIN_PATH_TABLE_DIRECT)
-                  : wide_keys ? HYB_JOIN_PATH_TABLE_HASH_WIDE : HYB_JOIN_PATH_TABLE_HASH;
-  if (probe_tiles) path |= use_span ? HYB_JOIN_PATH_PROBE_SPAN : params.fast ? HYB_JOIN_PATH_PROBE_TILE_LEAN : HYB_JOIN_PATH_PROBE_TILE;
-  if (dup_counts) path |= HYB_JOIN_PATH_RERUN;
-  context->timing.stats.path = path;
-
+  context->timing.stats.path = join_path_code(table_plan, probe_plan, probed, rerun);
   const auto handle = context->next_handle++;
   context->join_results.emplace(handle, std::move(result));
   *out_result = handle;
   return HYB_OK;
 }
+
 
 extern "C" {
 
@@ -2106,10 +2208,8 @@ int hyb_join_materialize(hyb_context* context, const hyb_join_side* side, uint32
   timing_begin(context);
   timing_kernel_begin(context);
   if (info.source.tile_count) {
-    const uint32_t grid = std::min<uint32_t>(info.source.tile_count, context->sm_count * 8);
-    join_materialize_kernel<<<grid, kJoinThreads, 0, context->stream>>>(info.source, chunk_id_base,
-                                                                        static_cast<long long*>(out_keys_device),
-                                                                        static_cast<long long*>(out_row_ids_device));
+    join_materialize_kernel<<<tile_grid(context, info.source.tile_count, 8), kJoinThreads, 0, context->stream>>>(
+        info.source, chunk_id_base, static_cast<long long*>(out_keys_device), static_cast<long long*>(out_row_ids_device));
     HYB_CUDA(cudaGetLastError());
   }
   timing_kernel_end(context);
@@ -2138,48 +2238,29 @@ static int partition_side(hyb_context* context, const hyb_join_side* side, uint3
   const uint32_t tiles = info.source.tile_count;
   // Same machinery as the probe: count per (partition, tile) -> exclusive scan -> ranked write. No table, no lookups.
   const size_t histogram_entries = size_t{partition_count} * std::max<uint32_t>(tiles, 1);
-  void* histogram = nullptr;
-  void* run_starts = nullptr;
-  void* control = nullptr;
-  void* offsets = nullptr;
-  HYB_TRY(device_alloc(context, sizeof(uint32_t) * histogram_entries, &histogram));
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * histogram_entries, &run_starts));
-  HYB_TRY(device_alloc(context, 64, &control));
-  HYB_TRY(device_alloc(context, sizeof(uint64_t) * (size_t{partition_count} + 1), &offsets));
+  DeviceScratch scratch(context);
+  uint32_t* histogram = nullptr;
+  unsigned long long* run_starts = nullptr;
+  uint32_t* control = nullptr;
+  unsigned long long* offsets = nullptr;
+  HYB_TRY(scratch.alloc_array(histogram_entries, &histogram));
+  HYB_TRY(scratch.alloc_array(histogram_entries, &run_starts));
+  HYB_TRY(scratch.alloc_array(16, &control));
+  HYB_TRY(scratch.alloc_array(size_t{partition_count} + 1, &offsets));
   HYB_CUDA(cudaMemsetAsync(control, 0, 64, stream));
-  auto* flags = static_cast<uint32_t*>(control);
-  auto* total_slot = reinterpret_cast<unsigned long long*>(flags + 4);
-  ProbeParams params{};
-  params.probe = info.source;
-  params.build = info.source;
-  params.mode = kModePartition;
-  params.partition_mask = partition_count - 1;
-  params.partition_count = partition_count;
-  params.unique_build = 1;
-  params.flags = flags;
-  params.histogram = static_cast<uint32_t*>(histogram);
-  params.run_starts = static_cast<const unsigned long long*>(run_starts);
-  params.overflow = flags + 2;
+  ProbeParams params = partition_params(info, partition_count, chunk_id_base, control, histogram, run_starts);
   params.out_build = static_cast<hyb_row_id*>(out_keys_device);
   params.out_probe = static_cast<hyb_row_id*>(out_row_ids_device);
   params.out_capacity = info.positions;
-  params.chunk_id_base = chunk_id_base;
-  int count_blocks = 1, write_blocks = 1;
-  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&count_blocks, join_probe_count_kernel<false>, kJoinThreads, 0));
+  int write_blocks = 1;
   HYB_CUDA(cudaFuncSetAttribute(join_partition_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(kPartitionStageBytes)));
   HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&write_blocks, join_partition_write_kernel, kJoinThreads, kPartitionStageBytes));
   uint32_t launches = 0;
   timing_kernel_begin(context);
   if (tiles) {
-    join_probe_count_kernel<false><<<std::min<uint32_t>(tiles, context->sm_count * std::max(count_blocks, 1)), kJoinThreads, 0, stream>>>(params);
-    HYB_CUDA(cudaGetLastError());
-    HYB_TRY(run_exclusive_scan(context, static_cast<uint32_t*>(histogram), static_cast<unsigned long long*>(run_starts),
-                               histogram_entries, total_slot));
-    join_partition_offsets_kernel<<<(partition_count + 1 + 127) / 128, 128, 0, stream>>>(
-        static_cast<const unsigned long long*>(run_starts), total_slot, partition_count, tiles,
-        static_cast<unsigned long long*>(offsets));
-    HYB_CUDA(cudaGetLastError());
+    HYB_TRY(count_partitions(context, params, tiles, reinterpret_cast<unsigned long long*>(control + 4), offsets,
+                             [&] { return launch_partition_count(context, params); }, no_write));
     launches += 3;
     if (exchange) {
       // The destinations depend on what every other rank sends: hand the counts to the host layer (one small
@@ -2206,8 +2287,7 @@ static int partition_side(hyb_context* context, const hyb_join_side* side, uint3
     if (tiles) timing_kernel_begin(context);
   }
   if (tiles) {
-    join_partition_write_kernel<<<std::min<uint32_t>(tiles, context->sm_count * std::max(write_blocks, 1)), kJoinThreads,
-                                  kPartitionStageBytes, stream>>>(params);
+    join_partition_write_kernel<<<tile_grid(context, tiles, write_blocks), kJoinThreads, kPartitionStageBytes, stream>>>(params);
     HYB_CUDA(cudaGetLastError());
     ++launches;
     timing_kernel_end(context);
@@ -2219,10 +2299,6 @@ static int partition_side(hyb_context* context, const hyb_join_side* side, uint3
   }
   timing_end(context, launches, info.positions * 16, info.positions, 0);
   HYB_CUDA(cudaStreamSynchronize(stream));  // local: the caller hands the buffers to NCCL; push: stores to peers are done
-  device_free(context, histogram);
-  device_free(context, run_starts);
-  device_free(context, control);
-  device_free(context, offsets);
   if (out_partition_offsets) {
     for (uint32_t p = 0; p <= partition_count; ++p) out_partition_offsets[p] = offsets_host[p];
   }
@@ -2338,33 +2414,58 @@ static int peer_count_side(hyb_context* context, DeviceScratch& scratch, const S
   HYB_TRY(scratch.alloc_array(16, &control));
   HYB_CUDA(cudaMemsetAsync(control, 0, 64, context->stream));
   HYB_CUDA(cudaMemsetAsync(offsets, 0, sizeof(unsigned long long) * (size_t{world} + 1), context->stream));
-  *params = ProbeParams{};
-  params->probe = info.source;
-  params->build = info.source;
-  params->mode = kModePartition;
-  params->partition_mask = world - 1;
-  params->partition_count = world;
-  params->unique_build = 1;
-  params->flags = control;
-  params->histogram = histogram;
-  params->run_starts = run_starts;
-  params->overflow = control + 2;
+  *params = partition_params(info, world, chunk_id_base, control, histogram, run_starts);
   params->out_capacity = ~0ull;
-  params->chunk_id_base = chunk_id_base;
   params->push_to_peers = 1;
   if (tiles) {
-    int count_blocks = 1;
-    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&count_blocks, join_probe_count_kernel<false>, kJoinThreads, 0));
-    join_probe_count_kernel<false><<<std::min<uint32_t>(tiles, context->sm_count * std::max(count_blocks, 1)), kJoinThreads, 0,
-                                     context->stream>>>(*params);
-    HYB_CUDA(cudaGetLastError());
-    HYB_TRY(run_exclusive_scan(context, histogram, run_starts, histogram_entries, reinterpret_cast<unsigned long long*>(control + 4)));
-    join_partition_offsets_kernel<<<1, 128, 0, context->stream>>>(run_starts, reinterpret_cast<unsigned long long*>(control + 4),
-                                                                  world, tiles, offsets);
-    HYB_CUDA(cudaGetLastError());
+    HYB_TRY(count_partitions(context, *params, tiles, reinterpret_cast<unsigned long long*>(control + 4), offsets,
+                             [&] { return launch_partition_count(context, *params); }, no_write));
   }
   *out_offsets = offsets;
   return HYB_OK;
+}
+
+// The radix width of a distributed join when the caller leaves it to the library: JoinHash's rule over the global build
+// side, raised until every rank owns a partition. The co-located and the exchanging path share it, so their results agree.
+static int32_t distributed_radix_bits(uint64_t global_build_rows, uint32_t world) {
+  int32_t radix_bits = std::max<int32_t>(calculate_radix_bits(global_build_rows), 0);
+  while ((1u << radix_bits) < world) ++radix_bits;
+  return radix_bits;
+}
+
+// Co-located shards: no rank's probe keys [min, max] overlap another rank's build keys. `bounds`: 8 words per rank as
+// peer_publish_bounds_kernel writes them (build min, max, has keys, rows; probe min, max, has keys, rows).
+static bool shards_colocated(const long long* bounds, uint32_t world) {
+  for (uint32_t r = 0; r < world; ++r) {
+    for (uint32_t other = 0; other < world; ++other) {
+      if (other == r || bounds[r * 8 + 6] == 0 || bounds[other * 8 + 2] == 0) continue;  // no probe keys / no build keys
+      if (bounds[r * 8 + 5] >= bounds[other * 8 + 0] && bounds[r * 8 + 4] <= bounds[other * 8 + 1]) return false;
+    }
+  }
+  return true;
+}
+
+// Bounds of the build keys this rank received, without another pass: they lie inside the union of the ranks' column
+// bounds (`key_info`: min, max, has keys per rank) and agree in their low log2(world) bits, which is what brought them
+// here. The min becomes the smallest value >= min with this rank's low bits, which keeps (key - min) a multiple of
+// 2^shift: a direct table indexed by (key - min) >> shift.
+static Table::KeyBounds received_key_bounds(const long long* key_info, uint32_t world, uint32_t rank) {
+  Table::KeyBounds bounds{};
+  for (uint32_t source = 0; source < world; ++source) {
+    if (key_info[source * 4 + 2] == 0) continue;
+    bounds.min = bounds.has_values ? std::min<long long>(bounds.min, key_info[source * 4 + 0]) : key_info[source * 4 + 0];
+    bounds.max = bounds.has_values ? std::max<long long>(bounds.max, key_info[source * 4 + 1]) : key_info[source * 4 + 1];
+    bounds.has_values = true;
+  }
+  if (!bounds.has_values) return bounds;
+  uint32_t shift = 0;
+  while ((1u << shift) < world) ++shift;
+  const long long mask = static_cast<long long>(world) - 1;
+  const long long aligned = bounds.min + ((static_cast<long long>(rank) - (bounds.min & mask)) & mask);
+  bounds.min = aligned;
+  bounds.max = std::max(bounds.max, aligned);
+  bounds.constant_low_bits = shift;
+  return bounds;
 }
 
 }  // namespace hyb
@@ -2410,8 +2511,8 @@ int hyb_join_hash_distributed(hyb_context* context, hyb_peer_group_t group_handl
   Table::KeyBounds side_bounds[2]{};
   if (context->options.join_colocated && !sides[0].filter && !sides[1].filter) {
     uint32_t bounds_launches = 0;
-    HYB_TRY(column_key_bounds(context, sides[0], build_side->column_id, &side_bounds[0], &bounds_launches));
-    HYB_TRY(column_key_bounds(context, sides[1], probe_side->column_id, &side_bounds[1], &bounds_launches));
+    HYB_TRY(column_key_bounds(context, sides[0], &side_bounds[0], &bounds_launches));
+    HYB_TRY(column_key_bounds(context, sides[1], &side_bounds[1], &bounds_launches));
     peer_publish_bounds_kernel<<<1, 32, 0, stream>>>(
         controls, rank, world, epoch, side_bounds[0].min, side_bounds[0].max, side_bounds[0].has_values ? 1 : 0,
         static_cast<long long>(sides[0].positions), side_bounds[1].min, side_bounds[1].max, side_bounds[1].has_values ? 1 : 0,
@@ -2421,20 +2522,12 @@ int hyb_join_hash_distributed(hyb_context* context, hyb_peer_group_t group_handl
     long long* h_bounds = reinterpret_cast<long long*>(group->h_counts);
     HYB_CUDA(cudaMemcpyAsync(h_bounds, group->control(rank)->side_bounds, sizeof(PeerControl::side_bounds), cudaMemcpyDeviceToHost, stream));
     HYB_CUDA(cudaStreamSynchronize(stream));
-    colocated = true;
-    uint64_t global_build_rows = 0;
-    for (uint32_t r = 0; r < world; ++r) {
-      global_build_rows += static_cast<uint64_t>(h_bounds[r * 8 + 3]);
-      for (uint32_t other = 0; other < world && colocated; ++other) {
-        if (other == r || h_bounds[r * 8 + 6] == 0 || h_bounds[other * 8 + 2] == 0) continue;  // no probe keys / no build keys
-        const bool disjoint = h_bounds[r * 8 + 5] < h_bounds[other * 8 + 0] || h_bounds[r * 8 + 4] > h_bounds[other * 8 + 1];
-        colocated = disjoint;
-      }
-    }
+    colocated = shards_colocated(h_bounds, world);
     if (colocated) {
       if (radix_bits < 0) {
-        radix_bits = std::max<int32_t>(calculate_radix_bits(global_build_rows), 0);
-        while ((1u << radix_bits) < world) ++radix_bits;  // the same rule as the exchanging path: results agree
+        uint64_t global_build_rows = 0;
+        for (uint32_t r = 0; r < world; ++r) global_build_rows += static_cast<uint64_t>(h_bounds[r * 8 + 3]);
+        radix_bits = distributed_radix_bits(global_build_rows, world);
       }
       for (int e = 1; e <= 4; ++e) HYB_CUDA(cudaEventRecord(group->events[e], stream));  // split_count_ms = the bounds exchange
       hyb_join_result_t local_result = 0;
@@ -2455,7 +2548,7 @@ int hyb_join_hash_distributed(hyb_context* context, hyb_peer_group_t group_handl
   HYB_TRY(peer_count_side(context, scratch, sides[1], world, probe_chunk_base, &params[1], &offsets[1]));
   Table::KeyBounds local_bounds{};
   uint32_t bounds_launches = 0;
-  HYB_TRY(column_key_bounds(context, sides[0], build_side->column_id, &local_bounds, &bounds_launches));
+  HYB_TRY(column_key_bounds(context, sides[0], &local_bounds, &bounds_launches));
   peer_publish_counts_kernel<<<1, 32 * kPeerMax, 0, stream>>>(controls, rank, world, epoch, offsets[0], offsets[1], local_bounds.min,
                                                               local_bounds.max, local_bounds.has_values ? 1 : 0);
   HYB_CUDA(cudaGetLastError());
@@ -2501,7 +2594,7 @@ int hyb_join_hash_distributed(hyb_context* context, hyb_peer_group_t group_handl
   uint32_t expected = 0;
   for (int side = 0; side < 2; ++side) {
     const uint32_t tiles = sides[side].source.tile_count;
-    grids[side] = tiles ? std::min<uint32_t>(tiles, context->sm_count * std::max(write_blocks, 1)) : 0;
+    grids[side] = tiles ? tile_grid(context, tiles, write_blocks) : 0;
     expected += grids[side];
   }
   HYB_CUDA(cudaMemsetAsync(group->d_arrivals, 0, sizeof(unsigned int), stream));
@@ -2530,34 +2623,13 @@ int hyb_join_hash_distributed(hyb_context* context, hyb_peer_group_t group_handl
     for (uint32_t source = 0; source < world; ++source) {
       for (uint32_t destination = 0; destination < world; ++destination) global_build += count_at(0, source, destination);
     }
-    radix_bits = std::max<int32_t>(calculate_radix_bits(global_build), 0);
-    while ((1u << radix_bits) < world) ++radix_bits;
+    radix_bits = distributed_radix_bits(global_build, world);
   }
   hyb_table_t tables[2];
   HYB_TRY(received_table(context, group, 0, received[0], &tables[0]));
   HYB_TRY(received_table(context, group, 1, received[1], &tables[1]));
-  {
-    // Bounds of the received build keys without another pass: they lie inside the union of the ranks' column bounds and
-    // agree in their low log2(world) bits (that is what brought them here) -> direct table indexed by (key - min) >> shift.
-    Table::KeyBounds bounds{};
-    for (uint32_t source = 0; source < world; ++source) {
-      if (key_info[source * 4 + 2] == 0) continue;
-      bounds.min = bounds.has_values ? std::min<long long>(bounds.min, key_info[source * 4 + 0]) : key_info[source * 4 + 0];
-      bounds.max = bounds.has_values ? std::max<long long>(bounds.max, key_info[source * 4 + 1]) : key_info[source * 4 + 1];
-      bounds.has_values = true;
-    }
-    if (bounds.has_values && received[0] > 0) {
-      uint32_t shift = 0;
-      while ((1u << shift) < world) ++shift;
-      // smallest value >= min with the low bits of this rank (keeps (key - min) a multiple of 2^shift)
-      const long long mask = static_cast<long long>(world) - 1;
-      const long long aligned = bounds.min + ((static_cast<long long>(rank) - (bounds.min & mask)) & mask);
-      bounds.min = aligned;
-      bounds.max = std::max(bounds.max, aligned);
-      bounds.constant_low_bits = shift;
-      find_table(context, tables[0])->key_bounds.emplace(0u, bounds);
-    }
-  }
+  const Table::KeyBounds bounds = received_key_bounds(key_info, world, rank);
+  if (bounds.has_values && received[0] > 0) find_table(context, tables[0])->key_bounds.emplace(0u, bounds);
   hyb_join_side local_build{tables[0], 0, 0}, local_probe{tables[1], 0, 0};
   hyb_join_result_t result_handle = 0;
   HYB_TRY(join_hash_locked(context, &local_build, &local_probe, HYB_JOIN_INNER, radix_bits, &result_handle));

@@ -5,7 +5,7 @@ guarantees — segment claims (chunk sizes, encodings, FoR offset widths), key f
 increasing, duplicates) and the hyb_join_path code an Inner join reports under each `TABLE_KINDS` setting. test_join_layouts.py checks all of them on
 the host segments, so an encoder change fails there instead of moving a GPU case to other kernels unnoticed.
 
-`predict_path` restates the table / kernel choice of hyb_join_hash (join.cu, "build" and "probe" of join_hash_locked)
+`predict_path` restates the table / kernel choice of hyb_join_hash (join.cu, `plan_join_table` and `plan_probe`)
 from those facts; test_gpu_join_paths.py asserts the hyb_join_path code the library reports against it.
 """
 from __future__ import annotations
@@ -624,7 +624,7 @@ def layout_facts(layout: JoinLayout, build_list=None, probe_list=None):
 
 
 def predict_table(build: SideFacts, probe: SideFacts, kind: str) -> tuple[int, int, bool, bool]:
-    """(table code, direct shift, direct, rank) as join_hash_locked chooses them."""
+    """(table code, direct shift, direct, rank) as plan_join_table chooses them."""
     table_option = TABLE_KINDS[kind][0]
     key_span = (build.key_max - build.key_min) & ((1 << 64) - 1)
     shift = build.low_bits
