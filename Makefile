@@ -16,9 +16,10 @@ COLUMN_SCAN_ORACLE := build/libcolumn_scan_oracle.so
 AGGREGATE_DISTINCT_ORACLE := build/libaggregate_distinct_oracle.so
 IN_SCAN_ORACLE := build/libin_scan_oracle.so
 EXPRESSION_SCAN_ORACLE := build/libexpression_scan_oracle.so
+JOIN_PREDICATES_ORACLE := build/libjoin_predicates_oracle.so
 
 all: $(LIB) $(TPCH_LIB) oracle $(COLUMN_SCAN_ORACLE) $(AGGREGATE_DISTINCT_ORACLE) $(IN_SCAN_ORACLE) \
-     $(EXPRESSION_SCAN_ORACLE)
+     $(EXPRESSION_SCAN_ORACLE) $(JOIN_PREDICATES_ORACLE)
 
 build/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p build
@@ -53,6 +54,19 @@ build/column_scan_check: tests/cpp/column_scan_check.cpp include/hyrise_b200.hpp
 	@mkdir -p build
 	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/column_scan_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
 		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
+
+# JoinHash with secondary predicates through the mirror on the GPU (the overload and its predicate flip).
+build/join_predicates_check: tests/cpp/join_predicates_check.cpp include/hyrise_b200.hpp include/hyrise_b200.h $(LIB)
+	@mkdir -p build
+	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/join_predicates_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
+		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
+
+# CPU restatement of JoinHash with secondary predicates on top of the CPU oracle's join steps (test infrastructure,
+# tests/join_predicates_oracle.py). No -ffast-math: the evaluator's comparisons must follow IEEE and C++'s conversions.
+$(JOIN_PREDICATES_ORACLE): tests/cpp/join_predicates_oracle.cpp oracle/oracle.cpp oracle/oracle.h include/hyrise_b200.h
+	@mkdir -p build
+	$(CXX) -O2 -std=c++17 -fPIC -Wall -Wextra -Wno-unused-parameter -Wno-unused-function -pthread -shared -o $@ \
+		tests/cpp/join_predicates_oracle.cpp
 
 # CPU restatement of ColumnVsColumnTableScanImpl on decoded numeric values (test infrastructure, tests/column_scan_oracle.py).
 # No -ffast-math: the comparisons must follow IEEE and C++'s arithmetic conversions exactly.

@@ -43,6 +43,7 @@ JOIN_PATH_TABLE_MASK = 0xF
 JOIN_PATH_PROBE_NONE, JOIN_PATH_PROBE_SPAN, JOIN_PATH_PROBE_TILE_LEAN, JOIN_PATH_PROBE_TILE = 0x00, 0x10, 0x20, 0x30
 JOIN_PATH_PROBE_MASK = 0xF0
 JOIN_PATH_RERUN = 0x100
+JOIN_PATH_SECONDARY = 0x200
 
 MAX_EXPR_NODES = 16
 MAX_GROUPBY_COLUMNS = 8
@@ -53,6 +54,7 @@ MAX_EXPRESSION_COLUMNS = 8
 MAX_EXPRESSION_TESTS = 16
 MAX_EXPRESSION_DEPTH = 8
 MAX_SORT_COLUMNS = 8
+MAX_JOIN_PREDICATES = 4
 SORT_KEY_AGGREGATE, SORT_KEY_COLUMN = range(2)  # hyb_aggregate_sort_key::kind
 INVALID_VALUE_ID = 0xFFFFFFFF
 DEFAULT_CHUNK_SIZE = 65535
@@ -128,6 +130,11 @@ class InPredicate(C.Structure):
 
 class JoinSide(C.Structure):
     _fields_ = [("table", C.c_uint64), ("column_id", C.c_uint32), ("filter", C.c_uint64)]
+
+
+class JoinPredicate(C.Structure):
+    _fields_ = [("build_column_id", C.c_uint32), ("probe_column_id", C.c_uint32), ("condition", C.c_int32),
+                ("reserved", C.c_uint32)]
 
 
 class ExprNode(C.Structure):
@@ -261,6 +268,8 @@ SYMBOLS = {
     "hyb_pos_list_copy": [_CTX, _U64, _U64, _U64, _P],
     "hyb_pos_list_free": [_CTX, _U64],
     "hyb_join_hash": [_CTX, C.POINTER(JoinSide), C.POINTER(JoinSide), _I32, _I32, C.POINTER(_U64)],
+    "hyb_join_hash_predicates": [_CTX, C.POINTER(JoinSide), C.POINTER(JoinSide), _I32, _I32, C.POINTER(JoinPredicate), _U32,
+                                 C.POINTER(_U64)],
     "hyb_join_result_info": [_CTX, _U64, C.POINTER(_U64), C.POINTER(_U32), C.POINTER(_I32)],
     "hyb_join_result_partition_offsets": [_CTX, _U64, _P],
     "hyb_join_result_copy": [_CTX, _U64, _U64, _U64, _P, _P],

@@ -1,4 +1,5 @@
-// Column-vs-column predicate tests (`left <op> right` in one row), used by the TableScan pipelines of scan.cu.
+// Column-vs-column predicate tests (`left <op> right` in one row), used by the TableScan pipelines of scan.cu; JoinHash's
+// secondary predicates (join.cu) compare a build row with a probe row through decode1 and compare1.
 //
 // Restates ColumnVsColumnTableScanImpl::_typed_scan_chunk_with_iterators and the two-iterator loop of
 // AbstractTableScanImpl::_scan_with_iterators<true> (abstract_table_scan_impl.hpp:56-84): a row matches iff neither side
@@ -23,6 +24,15 @@ enum PairCompare : uint32_t {
   kCompareFloat = 1,   // int x float, float x float: the integer rounded to the nearest float first
   kCompareDouble = 2   // anything with a double, float x double
 };
+
+// The common type of std::less<void> and friends on two numeric column types (C++'s usual arithmetic conversions):
+// TableScan's column pairs and JoinHash's secondary predicates.
+inline PairCompare pair_compare(int32_t left_type, int32_t right_type) {
+  const auto floating = [](int32_t type) { return type == HYB_TYPE_FLOAT32 || type == HYB_TYPE_FLOAT64; };
+  if (left_type == HYB_TYPE_FLOAT64 || right_type == HYB_TYPE_FLOAT64) return kCompareDouble;
+  if (floating(left_type) || floating(right_type)) return kCompareFloat;
+  return kCompareInt64;
+}
 
 // The per-chunk test of a column pair (ChunkTest stays the one-column test).
 struct PairTest {

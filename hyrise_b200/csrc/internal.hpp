@@ -160,6 +160,7 @@ struct JoinResult {
   hyb_row_id* d_probe = nullptr;
   uint64_t* d_partition_offsets = nullptr;  // partition_count + 1
   uint64_t capacity = 0;
+  bool secondary = false;                   // joined with secondary predicates (hyb_join_hash_predicates)
   std::vector<uint64_t> h_partition_offsets;
   bool host_valid = false;
   cudaStream_t stream = nullptr;

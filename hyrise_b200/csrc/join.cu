@@ -24,11 +24,14 @@
 //
 // Semi / Anti modes emit probe RowIDs only (probe_semi_anti); Left/Right emit NULL_ROW_ID partners for unmatched or
 // NULL probe keys (probe<keep_null_values = true>). NULL build keys are never inserted (join_hash.cpp:271-286).
+// Secondary predicates (hyb_join_hash_predicates) run a variant of the two tile kernels that evaluates them per candidate
+// (join_probe_secondary_count_kernel / join_probe_secondary_write_kernel).
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
 
+#include "column_pair.cuh"
 #include "device_utils.cuh"
 #include "internal.hpp"
 #include "peer.hpp"
@@ -637,6 +640,21 @@ __global__ void __launch_bounds__(kJoinThreads) exclusive_scan_kernel(const uint
 // ---------------------------------------------------------------------------------------------------------------------
 // Probe
 // ---------------------------------------------------------------------------------------------------------------------
+// One secondary predicate of hyb_join_hash_predicates: `build value <condition> probe value` in the common type of the
+// two columns.
+struct JoinPredicate {
+  const DevSegment* build;  // the build column's descriptors, one per chunk
+  const DevSegment* probe;  // the probe column's descriptors
+  int32_t condition;        // HYB_PRED_EQUALS .. HYB_PRED_GREATER_THAN_EQUALS
+  uint32_t compare;         // PairCompare
+};
+
+// The second argument of the *_secondary_* probe kernels (ProbeParams stays the other kernels' layout).
+struct SecondaryPredicates {
+  const JoinPredicate* predicates;  // device copy
+  uint32_t count;
+};
+
 struct ProbeParams {
   KeySource probe;
   KeySource build;                        // for position -> RowID of the build side
@@ -727,6 +745,146 @@ __device__ __forceinline__ uint32_t emitted_rows(const ProbeParams& params, uint
   return params.dup_counts[match];
 }
 
+// ---- secondary predicates (hyb_join_hash_predicates) -----------------------------------------------------------------
+// probe / probe_semi_anti with a MultiPredicateJoinEvaluator (join_hash_steps.hpp:690-748, :844-883): every candidate of
+// a probe row — a build row with its key — is tested against every predicate, one FieldComparator::compare each
+// (multi_predicate_join_evaluator.cpp): a NULL on either side fails, otherwise the comparator in the common type.
+// Candidates are never materialised: the count pass counts the passing ones; the write pass evaluates them again to
+// rank the row and, for Inner / Left / Right rows with passing candidates, a third time to store exactly those pairs.
+
+// One side's value of every predicate at one row, as the bits of each predicate's common type; bit i of `nulls`: NULL.
+struct PredicateValues {
+  unsigned long long bits[HYB_MAX_JOIN_PREDICATES];
+  uint32_t nulls;
+};
+
+// Returns true for NULL (a NULL_ROW_ID of a filter is NULL in every column).
+__device__ __forceinline__ bool predicate_value(const DevSegment* segments, uint32_t compare, hyb_row_id row,
+                                                unsigned long long& bits) {
+  if (row.chunk_id == HYB_INVALID_CHUNK_ID) return true;
+  const DevSegment& segment = segments[row.chunk_id];
+  if (compare == kCompareInt64) {
+    long long value;
+    if (decode1<AsInt64>(segment, row.chunk_offset, value)) return true;
+    bits = static_cast<unsigned long long>(value);
+  } else if (compare == kCompareFloat) {
+    float value;
+    if (decode1<AsFloat>(segment, row.chunk_offset, value)) return true;
+    bits = __float_as_uint(value);
+  } else {
+    double value;
+    if (decode1<AsDouble>(segment, row.chunk_offset, value)) return true;
+    bits = static_cast<unsigned long long>(__double_as_longlong(value));
+  }
+  return false;
+}
+
+// The probe row's values: decoded once per probe row and evaluation (secondary_resolved, write_passing_candidates). Not
+// inlined: the probe loops are unrolled 16 times.
+__device__ __noinline__ PredicateValues probe_predicate_values(const JoinPredicate* predicates, uint32_t count, hyb_row_id row) {
+  PredicateValues values{};
+#pragma unroll
+  for (uint32_t i = 0; i < HYB_MAX_JOIN_PREDICATES; ++i) {
+    if (i < count && predicate_value(predicates[i].probe, predicates[i].compare, row, values.bits[i])) values.nulls |= 1u << i;
+  }
+  return values;
+}
+
+// Whether the build row `row` passes every predicate against the probe row's values.
+__device__ __noinline__ bool candidate_passes(const JoinPredicate* predicates, uint32_t count, const PredicateValues probe,
+                                              hyb_row_id row) {
+#pragma unroll
+  for (uint32_t i = 0; i < HYB_MAX_JOIN_PREDICATES; ++i) {
+    if (i >= count) break;
+    if ((probe.nulls >> i) & 1u) return false;
+    const JoinPredicate predicate = predicates[i];
+    unsigned long long bits = 0;
+    if (predicate_value(predicate.build, predicate.compare, row, bits)) return false;
+    bool holds;
+    if (predicate.compare == kCompareInt64) {
+      holds = compare1(predicate.condition, static_cast<long long>(bits), static_cast<long long>(probe.bits[i]));
+    } else if (predicate.compare == kCompareFloat) {
+      holds = compare1(predicate.condition, __uint_as_float(static_cast<uint32_t>(bits)),
+                       __uint_as_float(static_cast<uint32_t>(probe.bits[i])));
+    } else {
+      holds = compare1(predicate.condition, __longlong_as_double(static_cast<long long>(bits)),
+                       __longlong_as_double(static_cast<long long>(probe.bits[i])));
+    }
+    if (!holds) return false;
+  }
+  return true;
+}
+
+// The word a probe row's key lookup leaves for the predicates: its candidates (the build position of a unique build
+// side, else the table slot whose position list holds them), or — no key match, or a NULL key — kEmitWithoutPartner for
+// the modes that keep such rows and kNoMatch for the others.
+__device__ __forceinline__ uint32_t secondary_candidates(const ProbeParams& params, uint32_t slot, uint32_t value, bool is_null) {
+  if (!is_null && slot != kNoMatch) return params.unique_build ? value : slot;
+  const int32_t mode = params.mode;
+  return (mode == HYB_JOIN_LEFT || mode == HYB_JOIN_RIGHT || mode == HYB_JOIN_ANTI_NULL_AS_FALSE) ? kEmitWithoutPartner : kNoMatch;
+}
+
+// RowID of a probe side's tile index `index` in its own table (a NULL_ROW_ID of a filter stays one).
+__device__ __forceinline__ hyb_row_id probe_row_id(const KeySource& source, const TileRef& ref, uint32_t index) {
+  if (source.tile_map) return hyb_row_id{ref.chunk, ref.row0 + index};
+  return source.filter[ref.first_position + index];
+}
+
+// Evaluates the candidates of one probe row. Returns the match word the write pass acts on — kNoMatch, kEmitWithoutPartner
+// (one row without a build partner; Semi / Anti: the probe row) or, when candidates pass in an Inner / Left / Right join,
+// the candidates themselves — and the probe row's output rows in `emit`.
+__device__ __forceinline__ uint32_t secondary_resolved(const ProbeParams& params, const SecondaryPredicates& secondary,
+                                                       uint32_t candidates, const TileRef& ref, uint32_t index, uint32_t& emit) {
+  emit = candidates == kEmitWithoutPartner ? 1u : 0u;
+  if (candidates == kNoMatch || candidates == kEmitWithoutPartner) return candidates;
+  const int32_t mode = params.mode;
+  const bool existence = mode == HYB_JOIN_SEMI || mode == HYB_JOIN_ANTI_NULL_AS_FALSE;  // the first passing one decides
+  const PredicateValues probe = probe_predicate_values(secondary.predicates, secondary.count, probe_row_id(params.probe, ref, index));
+  const bool unique = params.unique_build != 0;
+  const uint32_t count = unique ? 1u : params.dup_counts[candidates];
+  const unsigned long long first = unique ? 0ull : params.dup_offsets[candidates];
+  uint32_t passing = 0;
+  for (uint32_t j = 0; j < count; ++j) {
+    const uint32_t position = unique ? candidates : params.dup_positions[first + j];
+    if (candidate_passes(secondary.predicates, secondary.count, probe, position_to_row_id(params.build, position))) {
+      ++passing;
+      if (existence) break;
+    }
+  }
+  if (mode == HYB_JOIN_SEMI || mode == HYB_JOIN_ANTI_NULL_AS_FALSE) {
+    const bool kept = (passing != 0) == (mode == HYB_JOIN_SEMI);
+    emit = kept ? 1u : 0u;
+    return kept ? kEmitWithoutPartner : kNoMatch;
+  }
+  if (passing) {
+    emit = passing;
+    return candidates;
+  }
+  if (mode == HYB_JOIN_INNER) return kNoMatch;
+  emit = 1;  // Left / Right: one row with a NULL build partner where the pairs would have been
+  return kEmitWithoutPartner;
+}
+
+// The write pass of a probe row with passing candidates: those candidates, in build-row order, from `at` on.
+__device__ __forceinline__ void write_passing_candidates(const ProbeParams& params, const SecondaryPredicates& secondary,
+                                                         uint32_t candidates, hyb_row_id probe_row, unsigned long long at) {
+  const PredicateValues probe = probe_predicate_values(secondary.predicates, secondary.count, probe_row);
+  const bool unique = params.unique_build != 0;
+  const uint32_t count = unique ? 1u : params.dup_counts[candidates];
+  const unsigned long long first = unique ? 0ull : params.dup_offsets[candidates];
+  for (uint32_t j = 0; j < count; ++j) {
+    const hyb_row_id build_row = position_to_row_id(params.build, unique ? candidates : params.dup_positions[first + j]);
+    if (!candidate_passes(secondary.predicates, secondary.count, probe, build_row)) continue;
+    if (at >= params.out_capacity) {
+      *params.overflow = 1;
+      return;
+    }
+    st_stream_v2(params.out_build + at, build_row.chunk_id, build_row.chunk_offset);
+    st_stream_v2(params.out_probe + at, probe_row.chunk_id, probe_row.chunk_offset);
+    ++at;
+  }
+}
+
 template <uint32_t kCodec>
 __device__ __forceinline__ bool codec_key(const KeySource& source, const TileRef& ref, const DevSegment& segment, uint32_t index,
                                           uint32_t for_minimum, long long& key, bool& is_null) {
@@ -765,11 +923,13 @@ struct ChunkRows {
 // histogram held before the add — the number of rows this warp chunk emitted into the partition in earlier steps — plus
 // the emitting peers in lower lanes is the row's rank: lane order is probe order, so ranks reproduce the reference order.
 // kSource: 0 = decode + look up, storing nothing; 1 = decode + look up and store match/partition per probe slot (hash
-// tables: the write kernel must not repeat the random accesses); 2 = load what mode 1 stored.
-template <bool kRank, int kSource, uint32_t kCodec>
+// tables: the write kernel must not repeat the random accesses); 2 = load what mode 1 stored. kSecondary: the match
+// word is secondary_candidates' (stored as such) and the row's output comes from evaluating them.
+template <bool kRank, int kSource, uint32_t kCodec, bool kSecondary = false>
 __device__ __forceinline__ void probe_chunk(const ProbeParams& params, const TileRef& ref, const DevSegment& segment,
                                             uint32_t chunk0, size_t tile_slot0, uint32_t lane, bool build_has_nulls,
-                                            uint32_t* histogram, ChunkRows& rows) {
+                                            uint32_t* histogram, ChunkRows& rows,
+                                            const SecondaryPredicates& secondary = SecondaryPredicates{}) {
   const bool unique = params.unique_build != 0;
   const uint32_t lanes_below = (1u << lane) - 1u;
   uint32_t for_minimum = 0;
@@ -800,7 +960,11 @@ __device__ __forceinline__ void probe_chunk(const ProbeParams& params, const Til
       if (valid) {
         uint32_t value = 0;
         const uint32_t slot = (!is_null && params.table.slots) ? table_find(params.table, key, value) : kNoMatch;
-        match = probe_match_resolved(params, slot, value, is_null, build_has_nulls);
+        if constexpr (kSecondary) {
+          match = secondary_candidates(params, slot, value, is_null);
+        } else {
+          match = probe_match_resolved(params, slot, value, is_null, build_has_nulls);
+        }
       }
       partition = static_cast<uint32_t>(static_cast<unsigned long long>(key)) & params.partition_mask;
       if constexpr (kSource == 1) {
@@ -808,7 +972,12 @@ __device__ __forceinline__ void probe_chunk(const ProbeParams& params, const Til
         params.partitions[tile_slot0 + index] = static_cast<uint8_t>(partition);
       }
     }
-    const uint32_t emit = emitted_rows(params, match);
+    uint32_t emit;
+    if constexpr (kSecondary) {
+      match = secondary_resolved(params, secondary, match, ref, index, emit);
+    } else {
+      emit = emitted_rows(params, match);
+    }
     if constexpr (!kRank) {
       if (emit) atomicAdd(histogram + partition, emit);  // counting needs no order
       continue;
@@ -960,8 +1129,9 @@ __device__ __forceinline__ void probe_chunk_any_codec(const ProbeParams& params,
 }
 
 // Emitted rows per (partition, tile). kStore: also keep match/partition per probe slot for the write kernel.
-template <bool kStore>
-__global__ void __launch_bounds__(kJoinThreads, 5) join_probe_count_kernel(const ProbeParams params) {
+// kSecondary: the secondary predicates' variant (generic decoder, candidates evaluated per probe row).
+template <bool kStore, bool kSecondary>
+__device__ __forceinline__ void probe_count_tiles(const ProbeParams& params, const SecondaryPredicates& secondary) {
   __shared__ uint32_t s_histogram[kMaxPartitions];
   const bool build_has_nulls = params.flags[1] != 0;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -972,16 +1142,21 @@ __global__ void __launch_bounds__(kJoinThreads, 5) join_probe_count_kernel(const
     const DevSegment segment = params.probe.tile_map ? params.probe.segments[ref.chunk] : DevSegment{};
     const size_t tile_slot0 = static_cast<size_t>(tile) * kJoinTileRows;
     ChunkRows rows;
-    const uint32_t codec = tile_codec(params.probe, segment);
-    if (!kStore && fast_tile(params, codec)) {
-      if (ref.row0 + kJoinTileRows <= segment.row_count) {
-        probe_chunk_fast_any_codec<false, true>(params, ref, segment, codec, warp * kJoinRowsPerWarp, lane, s_histogram, rows);
-      } else {
-        probe_chunk_fast_any_codec<false, false>(params, ref, segment, codec, warp * kJoinRowsPerWarp, lane, s_histogram, rows);
-      }
+    if constexpr (kSecondary) {
+      probe_chunk<false, kStore ? 1 : 0, kCodecGeneric, true>(params, ref, segment, warp * kJoinRowsPerWarp, tile_slot0, lane,
+                                                             build_has_nulls, s_histogram, rows, secondary);
     } else {
-      probe_chunk_any_codec<false, kStore ? 1 : 0>(params, ref, segment, codec, warp * kJoinRowsPerWarp, tile_slot0, lane,
-                                                   build_has_nulls, s_histogram, rows);
+      const uint32_t codec = tile_codec(params.probe, segment);
+      if (!kStore && fast_tile(params, codec)) {
+        if (ref.row0 + kJoinTileRows <= segment.row_count) {
+          probe_chunk_fast_any_codec<false, true>(params, ref, segment, codec, warp * kJoinRowsPerWarp, lane, s_histogram, rows);
+        } else {
+          probe_chunk_fast_any_codec<false, false>(params, ref, segment, codec, warp * kJoinRowsPerWarp, lane, s_histogram, rows);
+        }
+      } else {
+        probe_chunk_any_codec<false, kStore ? 1 : 0>(params, ref, segment, codec, warp * kJoinRowsPerWarp, tile_slot0, lane,
+                                                     build_has_nulls, s_histogram, rows);
+      }
     }
     __syncthreads();
     for (uint32_t p = threadIdx.x; p < params.partition_count; p += kJoinThreads) {
@@ -991,10 +1166,21 @@ __global__ void __launch_bounds__(kJoinThreads, 5) join_probe_count_kernel(const
   }
 }
 
+template <bool kStore>
+__global__ void __launch_bounds__(kJoinThreads, 5) join_probe_count_kernel(const ProbeParams params) {
+  probe_count_tiles<kStore, false>(params, SecondaryPredicates{});
+}
+
+template <bool kStore>
+__global__ void __launch_bounds__(kJoinThreads, 3) join_probe_secondary_count_kernel(const ProbeParams params,
+                                                                                     const SecondaryPredicates secondary) {
+  probe_count_tiles<kStore, true>(params, secondary);
+}
+
 // Stable multi-split: every probe row's output position = start of its (partition, tile) run (exclusive scan of the
 // histogram) + rows of lower warp chunks of the tile in that partition + its rank inside the warp chunk.
-template <bool kStored>
-__global__ void __launch_bounds__(kJoinThreads, 3) join_probe_write_kernel(const ProbeParams params) {
+template <bool kStored, bool kSecondary>
+__device__ __forceinline__ void probe_write_tiles(const ProbeParams& params, const SecondaryPredicates& secondary) {
   __shared__ uint32_t s_warp_histogram[kJoinWarps][kMaxPartitions];
   __shared__ unsigned long long s_start[kJoinWarps][kMaxPartitions];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1013,14 +1199,17 @@ __global__ void __launch_bounds__(kJoinThreads, 3) join_probe_write_kernel(const
     const DevSegment segment = params.probe.tile_map ? params.probe.segments[ref.chunk] : DevSegment{};
     const size_t tile_slot0 = static_cast<size_t>(tile) * kJoinTileRows;
     ChunkRows rows;
-    const uint32_t codec = kStored ? kCodecGeneric : tile_codec(params.probe, segment);
-    const bool fast = !kStored && fast_tile(params, codec);
+    const uint32_t codec = (kStored || kSecondary) ? kCodecGeneric : tile_codec(params.probe, segment);
+    const bool fast = !kStored && !kSecondary && fast_tile(params, codec);
     if (fast) {
       if (ref.row0 + kJoinTileRows <= segment.row_count) {
         probe_chunk_fast_any_codec<true, true>(params, ref, segment, codec, warp * kJoinRowsPerWarp, lane, s_warp_histogram[warp], rows);
       } else {
         probe_chunk_fast_any_codec<true, false>(params, ref, segment, codec, warp * kJoinRowsPerWarp, lane, s_warp_histogram[warp], rows);
       }
+    } else if constexpr (kSecondary) {
+      probe_chunk<true, kStored ? 2 : 0, kCodecGeneric, true>(params, ref, segment, warp * kJoinRowsPerWarp, tile_slot0, lane,
+                                                             build_has_nulls, s_warp_histogram[warp], rows, secondary);
     } else {
       probe_chunk_any_codec<true, kStored ? 2 : 0>(params, ref, segment, codec, warp * kJoinRowsPerWarp, tile_slot0, lane,
                                                    build_has_nulls, s_warp_histogram[warp], rows);
@@ -1059,7 +1248,8 @@ __global__ void __launch_bounds__(kJoinThreads, 3) join_probe_write_kernel(const
 #pragma unroll
     for (int step = 0; step < kProbeSteps; ++step) {
       const uint32_t match = rows.match[step];
-      const uint32_t emit = emitted_rows(params, match);
+      // secondary predicates: the candidate loop below checks the capacity row by row
+      const uint32_t emit = kSecondary ? (match == kNoMatch ? 0u : 1u) : emitted_rows(params, match);
       if (emit == 0) continue;
       const uint32_t index = warp * kJoinRowsPerWarp + step * 32 + lane;
       const uint32_t partition = (rows.partitions[step >> 2] >> (8 * (step & 3))) & 0xFFu;
@@ -1079,6 +1269,8 @@ __global__ void __launch_bounds__(kJoinThreads, 3) join_probe_write_kernel(const
       if (match == kEmitWithoutPartner) {
         if (emit_build) st_stream_v2(params.out_build + at, HYB_INVALID_CHUNK_ID, HYB_INVALID_CHUNK_OFFSET);
         st_stream_v2(params.out_probe + at, probe_row.chunk_id, probe_row.chunk_offset);
+      } else if constexpr (kSecondary) {
+        write_passing_candidates(params, secondary, match, probe_row, at);
       } else if (unique) {
         const hyb_row_id build_row = position_to_row_id(params.build, match);
         st_stream_v2(params.out_build + at, build_row.chunk_id, build_row.chunk_offset);
@@ -1094,6 +1286,19 @@ __global__ void __launch_bounds__(kJoinThreads, 3) join_probe_write_kernel(const
     }
     __syncthreads();
   }
+}
+
+template <bool kStored>
+__global__ void __launch_bounds__(kJoinThreads, 3) join_probe_write_kernel(const ProbeParams params) {
+  probe_write_tiles<kStored, false>(params, SecondaryPredicates{});
+}
+
+// (two CTAs per SM: at the 80 registers of three the candidate loops spilled 104-184 bytes; at 128 the direct-table
+// variant does not spill and the hash-table variant, kStored, still spills 24 bytes)
+template <bool kStored>
+__global__ void __launch_bounds__(kJoinThreads, 2) join_probe_secondary_write_kernel(const ProbeParams params,
+                                                                                     const SecondaryPredicates secondary) {
+  probe_write_tiles<kStored, true>(params, secondary);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1633,12 +1838,17 @@ struct SideInfo {
   uint64_t positions = 0;
 };
 
+// A column's type on a join side (a table without chunks has none: its columns read as int32).
+static int32_t side_column_type(const SideInfo& side, uint32_t column_id) {
+  return side.table->chunk_count() ? side.table->column_types[column_id] : HYB_TYPE_INT32;
+}
+
 static int prepare_side(hyb_context* context, const hyb_join_side* side, SideInfo* out) {
   out->table = find_table(context, side->table);
   HYB_CHECK(out->table, HYB_ERR_NOT_FOUND, "unknown table handle");
   HYB_CHECK(side->column_id < out->table->column_count, HYB_ERR_INVALID, "join column out of range");
   out->column_id = side->column_id;
-  out->data_type = out->table->chunk_count() ? out->table->column_types[side->column_id] : HYB_TYPE_INT32;
+  out->data_type = side_column_type(*out, side->column_id);
   HYB_CHECK(out->data_type == HYB_TYPE_INT32 || out->data_type == HYB_TYPE_INT64, HYB_ERR_UNSUPPORTED,
             "JoinHash on the device supports int32/int64 key columns; other key types run on the CPU operator");
   HYB_TRY(sync_table_descriptors(context, out->table));
@@ -1860,11 +2070,12 @@ struct ProbePlan {
   uint32_t tile_fast = 0;  // ProbeParams::fast of the tile kernels, whose lean path knows the direct table only
 };
 
-static ProbePlan plan_probe(const JoinTablePlan& table, const SideInfo& probe, int32_t mode, const ContextOptions& options) {
+static ProbePlan plan_probe(const JoinTablePlan& table, const SideInfo& probe, int32_t mode, bool secondary,
+                            const ContextOptions& options) {
   // Lean path of the case that dominates (Inner, dense unique build side): 1 = int32 keys on both sides, 2 = int64 probe
-  // keys against a (possibly shifted) direct table.
+  // keys against a (possibly shifted) direct table. Secondary predicates take the generic loop only.
   const uint32_t fast =
-      (mode == HYB_JOIN_INNER && table.direct)
+      (mode == HYB_JOIN_INNER && table.direct && !secondary)
           ? ((table.direct_shift == 0 && !table.wide) ? 1u : ((!table.rank && probe.data_type == HYB_TYPE_INT64) ? 2u : 0u))
           : 0u;
   ProbePlan plan;
@@ -1883,11 +2094,83 @@ static ProbePlan plan_probe(const JoinTablePlan& table, const SideInfo& probe, i
   return plan;
 }
 
+// Compulsory traffic of one column of a join side (SURVEY.md §8d): the column once, or a PosList's rows of it.
+static uint64_t join_column_bytes(const SideInfo& side, uint32_t column_id) {
+  if (side.filter) return side.positions * data_type_size(side_column_type(side, column_id));
+  uint64_t bytes = 0;
+  for (uint32_t chunk = 0; chunk < side.table->chunk_count(); ++chunk) {
+    const auto& segment = side.table->segments[size_t{chunk} * side.table->column_count + column_id];
+    bytes += segment.encoding == HYB_ENC_UNENCODED ? data_type_size(segment.data_type) * segment.row_count
+                                                   : vector_bytes(segment.vector_type, segment.bit_width, segment.row_count);
+    if (segment.encoding == HYB_ENC_FRAME_OF_REFERENCE) {
+      bytes += sizeof(int32_t) * ((segment.row_count + HYB_FOR_BLOCK_SIZE - 1) / HYB_FOR_BLOCK_SIZE);
+    }
+  }
+  return bytes;
+}
+
+// ... of one side's keys: the key column once, or a PosList's RowIDs and keys.
+static uint64_t join_key_bytes(const SideInfo& side) {
+  return join_column_bytes(side, side.column_id) + (side.filter ? side.positions * sizeof(hyb_row_id) : 0);
+}
+
+// The secondary predicates of a call (hyb_join_hash_predicates): checked, typed and copied to the device.
+struct SecondaryPlan {
+  SecondaryPredicates device{};     // count == 0: none
+  uint64_t algorithmic_bytes = 0;   // every distinct secondary column of both sides once
+};
+
+static int prepare_secondary(hyb_context* context, DeviceScratch& scratch, const SideInfo& build, const SideInfo& probe,
+                             const hyb_join_predicate* predicates, uint32_t count, SecondaryPlan* out) {
+  if (count == 0) return HYB_OK;
+  HYB_CHECK(!build.table->position_payload && !probe.table->position_payload, HYB_ERR_UNSUPPORTED,
+            "secondary join predicates read the columns of the rows they join; received exchange tuples stand for "
+            "another table's rows");
+  std::vector<JoinPredicate> host(count);
+  std::vector<uint32_t> build_columns, probe_columns;
+  for (uint32_t i = 0; i < count; ++i) {
+    const hyb_join_predicate& predicate = predicates[i];
+    HYB_CHECK(predicate.reserved == 0, HYB_ERR_INVALID, "hyb_join_predicate.reserved must be 0");
+    HYB_CHECK(predicate.build_column_id < build.table->column_count && predicate.probe_column_id < probe.table->column_count,
+              HYB_ERR_INVALID, "secondary join predicate column out of range");
+    HYB_CHECK(predicate.condition >= HYB_PRED_EQUALS && predicate.condition <= HYB_PRED_GREATER_THAN_EQUALS, HYB_ERR_INVALID,
+              "secondary join predicates take =, !=, <, <=, >, >= (condition " + std::to_string(predicate.condition) + ")");
+    const int32_t build_type = side_column_type(build, predicate.build_column_id);
+    const int32_t probe_type = side_column_type(probe, predicate.probe_column_id);
+    const bool strings = build_type == HYB_TYPE_STRING;
+    // multi_predicate_join_evaluator.cpp: Fail("Types of columns cannot be compared")
+    HYB_CHECK(strings == (probe_type == HYB_TYPE_STRING), HYB_ERR_INVALID, "Types of columns cannot be compared");
+    HYB_CHECK(!strings, HYB_ERR_UNSUPPORTED,
+              "string secondary join predicates need a dictionary translation per chunk pair; they run on the CPU operator");
+    host[i].build = build.table->d_segments + size_t{predicate.build_column_id} * build.table->chunk_count();
+    host[i].probe = probe.table->d_segments + size_t{predicate.probe_column_id} * probe.table->chunk_count();
+    host[i].condition = predicate.condition;
+    host[i].compare = pair_compare(build_type, probe_type);
+    const auto count_column = [&](std::vector<uint32_t>& seen, const SideInfo& side, uint32_t column) {
+      if (std::find(seen.begin(), seen.end(), column) != seen.end()) return;
+      seen.push_back(column);
+      out->algorithmic_bytes += join_column_bytes(side, column);
+    };
+    count_column(build_columns, build, predicate.build_column_id);
+    count_column(probe_columns, probe, predicate.probe_column_id);
+  }
+  JoinPredicate* device = nullptr;
+  HYB_TRY(scratch.alloc_array(count, &device));
+  // pageable source: the copy is staged before cudaMemcpyAsync returns
+  HYB_CUDA(cudaMemcpyAsync(device, host.data(), sizeof(JoinPredicate) * count, cudaMemcpyHostToDevice, context->stream));
+  out->device = SecondaryPredicates{device, count};
+  return HYB_OK;
+}
+
 // What every probe pass of one join shares.
 struct ProbeSetup {
   ProbeParams params{};  // the tile kernels' parameters; each pass fills in its output blocks
   void (*count_kernel)(const ProbeParams) = nullptr;
   void (*write_kernel)(const ProbeParams) = nullptr;
+  // secondary predicates: these tile kernels run instead, with `secondary` as their second argument
+  SecondaryPredicates secondary{};
+  void (*secondary_count_kernel)(const ProbeParams, const SecondaryPredicates) = nullptr;
+  void (*secondary_write_kernel)(const ProbeParams, const SecondaryPredicates) = nullptr;
   uint32_t count_grid = 1, write_grid = 1;
   KeySource span_source{};  // the span kernels: the probe side in kSpanRows-row spans
   bool rank = false;        // span kernel variants
@@ -1896,8 +2179,8 @@ struct ProbeSetup {
 };
 
 static int prepare_probe(hyb_context* context, DeviceScratch& scratch, const JoinTablePlan& plan, const ProbePlan& probe_plan,
-                         const SideInfo& build, const SideInfo& probe, int32_t mode, uint32_t partition_count,
-                         const HashTable& table, uint32_t* control, ProbeSetup* out) {
+                         const SecondaryPlan& secondary, const SideInfo& build, const SideInfo& probe, int32_t mode,
+                         uint32_t partition_count, const HashTable& table, uint32_t* control, ProbeSetup* out) {
   out->span_source = probe.source;
   if (probe_plan.span) HYB_TRY(get_tile_map(context, probe.table, kSpanRows, &out->span_source.tile_map, &out->span_source.tile_count));
   // Hash tables: the count kernel keeps match + partition per probe slot so that the write kernel does not repeat the
@@ -1907,8 +2190,16 @@ static int prepare_probe(hyb_context* context, DeviceScratch& scratch, const Joi
   out->count_kernel = store_matches ? join_probe_count_kernel<true> : join_probe_count_kernel<false>;
   out->write_kernel = store_matches ? join_probe_write_kernel<true> : join_probe_write_kernel<false>;
   int count_blocks = 1, write_blocks = 1;
-  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&count_blocks, out->count_kernel, kJoinThreads, 0));
-  HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&write_blocks, out->write_kernel, kJoinThreads, 0));
+  out->secondary = secondary.device;
+  if (secondary.device.count) {
+    out->secondary_count_kernel = store_matches ? join_probe_secondary_count_kernel<true> : join_probe_secondary_count_kernel<false>;
+    out->secondary_write_kernel = store_matches ? join_probe_secondary_write_kernel<true> : join_probe_secondary_write_kernel<false>;
+    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&count_blocks, out->secondary_count_kernel, kJoinThreads, 0));
+    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&write_blocks, out->secondary_write_kernel, kJoinThreads, 0));
+  } else {
+    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&count_blocks, out->count_kernel, kJoinThreads, 0));
+    HYB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&write_blocks, out->write_kernel, kJoinThreads, 0));
+  }
   const uint32_t probe_tiles = probe.source.tile_count;
   out->count_grid = tile_grid(context, probe_tiles, count_blocks);
   out->write_grid = tile_grid(context, probe_tiles, write_blocks);
@@ -1939,6 +2230,19 @@ static int prepare_probe(hyb_context* context, DeviceScratch& scratch, const Joi
   params.flags = control;
   params.run_starts = run_starts;
   params.overflow = control + 2;
+  return HYB_OK;
+}
+
+// One pass of the tile kernels (count or write) over setup.params: the secondary predicates' variant when there are any.
+static int launch_tile_pass(hyb_context* context, const ProbeSetup& setup, bool write) {
+  const uint32_t grid = write ? setup.write_grid : setup.count_grid;
+  if (setup.secondary.count) {
+    (write ? setup.secondary_write_kernel : setup.secondary_count_kernel)<<<grid, kJoinThreads, 0, context->stream>>>(
+        setup.params, setup.secondary);
+  } else {
+    (write ? setup.write_kernel : setup.count_kernel)<<<grid, kJoinThreads, 0, context->stream>>>(setup.params);
+  }
+  HYB_CUDA(cudaGetLastError());
   return HYB_OK;
 }
 
@@ -1985,7 +2289,7 @@ static int run_probe_pass(hyb_context* context, DeviceScratch& scratch, ProbeSet
     if (span) {
       count_spans<<<tiles, kSpanThreads, counter_bytes, stream>>>(span_params, fine_counts);
     } else {
-      setup.count_kernel<<<setup.count_grid, kJoinThreads, 0, stream>>>(params);
+      HYB_TRY(launch_tile_pass(context, setup, false));
     }
     HYB_CUDA(cudaGetLastError());
     return HYB_OK;
@@ -1998,7 +2302,7 @@ static int run_probe_pass(hyb_context* context, DeviceScratch& scratch, ProbeSet
     if (span) {
       write_spans<<<tiles, kSpanThreads, write_bytes, stream>>>(span_params, fine_counts);
     } else {
-      setup.write_kernel<<<setup.write_grid, kJoinThreads, 0, stream>>>(params);
+      HYB_TRY(launch_tile_pass(context, setup, true));
     }
     HYB_CUDA(cudaGetLastError());
     return HYB_OK;
@@ -2039,8 +2343,7 @@ static int rerun_with_duplicates(hyb_context* context, DeviceScratch& scratch, c
   params.dup_counts = dup_counts;
   params.dup_offsets = dup_offsets;
   params.dup_positions = dup_positions;
-  setup.count_kernel<<<setup.count_grid, kJoinThreads, 0, stream>>>(params);
-  HYB_CUDA(cudaGetLastError());
+  HYB_TRY(launch_tile_pass(context, setup, false));
   HYB_TRY(run_exclusive_scan(context, params.histogram, const_cast<unsigned long long*>(params.run_starts),
                              size_t{params.partition_count} * params.probe.tile_count, setup.total));
   *launches += 2;
@@ -2054,26 +2357,12 @@ static int rerun_with_duplicates(hyb_context* context, DeviceScratch& scratch, c
   return HYB_OK;
 }
 
-// Compulsory traffic of one side's keys (SURVEY.md §8d): the key column once, or a PosList's RowIDs and keys.
-static uint64_t join_key_bytes(const SideInfo& side) {
-  if (side.filter) return side.positions * (sizeof(hyb_row_id) + data_type_size(side.data_type));
-  uint64_t bytes = 0;
-  for (uint32_t chunk = 0; chunk < side.table->chunk_count(); ++chunk) {
-    const auto& segment = side.table->segments[size_t{chunk} * side.table->column_count + side.column_id];
-    bytes += segment.encoding == HYB_ENC_UNENCODED ? data_type_size(segment.data_type) * segment.row_count
-                                                   : vector_bytes(segment.vector_type, segment.bit_width, segment.row_count);
-    if (segment.encoding == HYB_ENC_FRAME_OF_REFERENCE) {
-      bytes += sizeof(int32_t) * ((segment.row_count + HYB_FOR_BLOCK_SIZE - 1) / HYB_FOR_BLOCK_SIZE);
-    }
-  }
-  return bytes;
-}
-
 // The hyb_join_path code of a join: its table kind, the probe kernels (when there were probe rows) and the rerun.
-static uint32_t join_path_code(const JoinTablePlan& table, const ProbePlan& probe, bool probed, bool rerun) {
+static uint32_t join_path_code(const JoinTablePlan& table, const ProbePlan& probe, bool probed, bool rerun, bool secondary) {
   uint32_t path = table.kind;
   if (probed) path |= probe.span ? HYB_JOIN_PATH_PROBE_SPAN : probe.tile_fast ? HYB_JOIN_PATH_PROBE_TILE_LEAN : HYB_JOIN_PATH_PROBE_TILE;
   if (rerun) path |= HYB_JOIN_PATH_RERUN;
+  if (secondary) path |= HYB_JOIN_PATH_SECONDARY;
   return path;
 }
 
@@ -2109,10 +2398,12 @@ static ProbeParams partition_params(const SideInfo& side, uint32_t partition_cou
 
 using namespace hyb;
 
-// hyb_join_hash with context->mutex held (hyb_join_hash_distributed joins the received tuples through it).
+// hyb_join_hash / hyb_join_hash_predicates with context->mutex held (hyb_join_hash_distributed joins the received tuples
+// through it).
 static int join_hash_locked(hyb_context* context, const hyb_join_side* build_side, const hyb_join_side* probe_side, int32_t mode,
                             int32_t radix_bits, hyb_join_result_t* out_result, uint32_t build_chunk_base = 0,
-                            uint32_t probe_chunk_base = 0) {
+                            uint32_t probe_chunk_base = 0, const hyb_join_predicate* predicates = nullptr,
+                            uint32_t predicate_count = 0) {
   SideInfo build, probe;
   HYB_TRY(prepare_side(context, build_side, &build));
   HYB_TRY(prepare_side(context, probe_side, &probe));
@@ -2127,6 +2418,8 @@ static int join_hash_locked(hyb_context* context, const hyb_join_side* build_sid
   cudaStream_t stream = context->stream;
   uint32_t launches = 0;
   DeviceScratch scratch(context);  // every scratch block of this call goes back to the cache on every exit path
+  SecondaryPlan secondary;
+  HYB_TRY(prepare_secondary(context, scratch, build, probe, predicates, predicate_count, &secondary));
   timing_begin(context);
 
   Table::KeyBounds bounds{};
@@ -2143,6 +2436,7 @@ static int join_hash_locked(hyb_context* context, const hyb_join_side* build_sid
   result->probe_table = probe_side->table;
   result->radix_bits = radix_bits;
   result->partition_count = partition_count;
+  result->secondary = secondary.device.count != 0;
   result->stream = stream;
   result->owner = context;
   void* partition_offsets = nullptr;
@@ -2150,9 +2444,10 @@ static int join_hash_locked(hyb_context* context, const hyb_join_side* build_sid
   result->d_partition_offsets = static_cast<uint64_t*>(partition_offsets);
   HYB_CUDA(cudaMemsetAsync(partition_offsets, 0, sizeof(uint64_t) * (size_t{partition_count} + 2), stream));
 
-  const ProbePlan probe_plan = plan_probe(table_plan, probe, mode, context->options);
+  const ProbePlan probe_plan = plan_probe(table_plan, probe, mode, secondary.device.count != 0, context->options);
   ProbeSetup setup;
-  HYB_TRY(prepare_probe(context, scratch, table_plan, probe_plan, build, probe, mode, partition_count, table, control, &setup));
+  HYB_TRY(prepare_probe(context, scratch, table_plan, probe_plan, secondary, build, probe, mode, partition_count, table, control,
+                        &setup));
   const bool probed = probe.source.tile_count != 0;
   // With a unique build side every probe row emits at most one output row: probe.positions rows always suffice.
   if (probed) HYB_TRY(run_probe_pass(context, scratch, setup, probe_plan.span, probe.positions, result.get(), &launches));
@@ -2160,12 +2455,13 @@ static int join_hash_locked(hyb_context* context, const hyb_join_side* build_sid
   uint32_t host_control[8] = {};
   HYB_CUDA(cudaMemcpyAsync(host_control, control, sizeof(host_control), cudaMemcpyDeviceToHost, stream));
   HYB_CUDA(cudaStreamSynchronize(stream));  // the only host round trip of the operator (unique build side)
-  const bool rerun = host_control[0] != 0 && !semi_or_anti && probed;
+  // Semi / Anti joins need every build row of a key only when its candidates are evaluated
+  const bool rerun = host_control[0] != 0 && (!semi_or_anti || secondary.device.count) && probed;
   if (rerun) HYB_TRY(rerun_with_duplicates(context, scratch, table_plan, build, table, setup, result.get(), &launches));
 
-  timing_end(context, launches, join_key_bytes(build) + join_key_bytes(probe), probe.positions, 0);
+  timing_end(context, launches, join_key_bytes(build) + join_key_bytes(probe) + secondary.algorithmic_bytes, probe.positions, 0);
   timing_output_count(context, result->d_partition_offsets + partition_count, semi_or_anti ? 8 : 16);
-  context->timing.stats.path = join_path_code(table_plan, probe_plan, probed, rerun);
+  context->timing.stats.path = join_path_code(table_plan, probe_plan, probed, rerun, secondary.device.count != 0);
   const auto handle = context->next_handle++;
   context->join_results.emplace(handle, std::move(result));
   *out_result = handle;
@@ -2185,6 +2481,25 @@ int hyb_join_hash(hyb_context* context, const hyb_join_side* build_side, const h
   DeviceGuard guard(context->device);
   std::lock_guard<std::mutex> lock(context->mutex);
   return join_hash_locked(context, build_side, probe_side, mode, radix_bits, out_result);
+}
+
+int hyb_join_hash_predicates(hyb_context* context, const hyb_join_side* build_side, const hyb_join_side* probe_side, int32_t mode,
+                             int32_t radix_bits, const hyb_join_predicate* predicates, uint32_t predicate_count,
+                             hyb_join_result_t* out_result) {
+  HYB_CHECK(context && build_side && probe_side && out_result && (predicates || predicate_count == 0), HYB_ERR_INVALID,
+            "NULL argument");
+  *out_result = 0;
+  HYB_CHECK(mode == HYB_JOIN_INNER || mode == HYB_JOIN_LEFT || mode == HYB_JOIN_RIGHT || mode == HYB_JOIN_SEMI ||
+                mode == HYB_JOIN_ANTI_NULL_AS_TRUE || mode == HYB_JOIN_ANTI_NULL_AS_FALSE,
+            HYB_ERR_UNSUPPORTED, "JoinMode not supported by JoinHash");
+  HYB_CHECK(predicate_count <= HYB_MAX_JOIN_PREDICATES, HYB_ERR_UNSUPPORTED,
+            "more than " + std::to_string(HYB_MAX_JOIN_PREDICATES) + " secondary join predicates");
+  // JoinHash::supports (join_hash.cpp:36-44): no AntiNullAsTrue with secondary predicates
+  HYB_CHECK(predicate_count == 0 || mode != HYB_JOIN_ANTI_NULL_AS_TRUE, HYB_ERR_UNSUPPORTED,
+            "AntiNullAsTrue joins with secondary predicates are not supported by JoinHash");
+  DeviceGuard guard(context->device);
+  std::lock_guard<std::mutex> lock(context->mutex);
+  return join_hash_locked(context, build_side, probe_side, mode, radix_bits, out_result, 0, 0, predicates, predicate_count);
 }
 
 int hyb_join_side_positions(hyb_context* context, const hyb_join_side* side, uint64_t* out_positions) {
@@ -2792,6 +3107,8 @@ int hyb_join_result_output_chunks(hyb_context* context, hyb_join_result_t handle
   std::lock_guard<std::mutex> lock(context->mutex);
   auto* result = find_join_result(context, handle);
   HYB_CHECK(result, HYB_ERR_NOT_FOUND, "unknown join result handle");
+  // probe() cuts its slices every PROBE_SIZE_PER_CHUNK probe elements, which secondary predicates decouple from the rows
+  HYB_CHECK(!result->secondary, HYB_ERR_UNSUPPORTED, "output chunks of a join with secondary predicates");
   HYB_TRY(ensure_join_host(context, result));
   // probe(): one PosList per non-empty partition and PROBE_SIZE_PER_CHUNK slice of it (join_hash_steps.hpp:47, :644-655)
   constexpr uint64_t kProbeSizePerChunk = uint64_t{HYB_DEFAULT_CHUNK_SIZE} * 2;

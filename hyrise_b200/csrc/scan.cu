@@ -1530,14 +1530,6 @@ static int prepare_pair_tests(hyb_context* context, const Table* table, const hy
   return HYB_OK;
 }
 
-// The common type of std::less<void> and friends on two numeric column types (C++'s usual arithmetic conversions).
-static PairCompare pair_compare(int32_t left_type, int32_t right_type) {
-  const auto floating = [](int32_t type) { return type == HYB_TYPE_FLOAT32 || type == HYB_TYPE_FLOAT64; };
-  if (left_type == HYB_TYPE_FLOAT64 || right_type == HYB_TYPE_FLOAT64) return kCompareDouble;
-  if (floating(left_type) || floating(right_type)) return kCompareFloat;
-  return kCompareInt64;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // [NOT] IN on a numeric column: per-chunk tests from the list's intervals. A dictionary chunk maps every interval [lo, hi]
 // to the value-IDs [lower_bound(lo), upper_bound(hi)) of its device-resident dictionary; the ranges are sorted and

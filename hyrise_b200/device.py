@@ -584,12 +584,20 @@ class DeviceContext:
 
     def join_hash(self, build: DeviceTable, build_column: int, probe: DeviceTable, probe_column: int, mode: int,
                   radix_bits: int = -1, build_filter: DevicePosList | None = None,
-                  probe_filter: DevicePosList | None = None) -> DeviceJoinResult:
+                  probe_filter: DevicePosList | None = None, secondary=None) -> DeviceJoinResult:
+        """hyb_join_hash; with `secondary` = [(build column, probe column, condition), ...] (`build value <condition>
+        probe value`, the list may be empty) hyb_join_hash_predicates."""
         build_side = capi.JoinSide(build.handle, build_column, build_filter.handle if build_filter else 0)
         probe_side = capi.JoinSide(probe.handle, probe_column, probe_filter.handle if probe_filter else 0)
         handle = C.c_uint64()
-        check(self.lib.hyb_join_hash(self.ptr, C.byref(build_side), C.byref(probe_side), mode, radix_bits,
-                                     C.byref(handle)))
+        if secondary is None:
+            check(self.lib.hyb_join_hash(self.ptr, C.byref(build_side), C.byref(probe_side), mode, radix_bits,
+                                         C.byref(handle)))
+        else:
+            predicates = (capi.JoinPredicate * max(len(secondary), 1))(
+                *[capi.JoinPredicate(build_col, probe_col, condition, 0) for build_col, probe_col, condition in secondary])
+            check(self.lib.hyb_join_hash_predicates(self.ptr, C.byref(build_side), C.byref(probe_side), mode, radix_bits,
+                                                    predicates, len(secondary), C.byref(handle)))
         semi_or_anti = mode in (capi.JOIN_SEMI, capi.JOIN_ANTI_NULL_AS_TRUE, capi.JOIN_ANTI_NULL_AS_FALSE)
         return DeviceJoinResult(self, handle.value, not semi_or_anti)
 

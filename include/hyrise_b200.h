@@ -527,6 +527,41 @@ typedef struct hyb_join_side {
 int hyb_join_hash(hyb_context* context, const hyb_join_side* build, const hyb_join_side* probe, int32_t mode,
                   int32_t radix_bits, hyb_join_result_t* out_result);
 
+/*
+ * Secondary join predicates: `build.key = probe.key AND build.<build_column_id> <condition> probe.<probe_column_id> AND
+ * ...` (JoinHash's OperatorJoinPredicates after the primary one, join_hash_steps.hpp:690-748, :844-883; the comparison
+ * of MultiPredicateJoinEvaluator, multi_predicate_join_evaluator.cpp). A predicate reads `build value <condition> probe
+ * value`; a caller that swaps the inputs flips each predicate's columns and condition (join_hash.cpp:158-165,
+ * hyb_flip_predicate_condition).
+ *   - condition: =, !=, <, <=, >, >=. A candidate (a build row with the probe row's key) passes when every predicate holds.
+ *   - Columns: int32, int64, float or double, in any pairing, compared in C++'s common type as hyb_table_scan_columns
+ *     compares (int x int in int64, int x float in float, anything with a double in double). NaN fails every condition
+ *     but !=; -0.0 equals +0.0. A NULL on either side makes the predicate false; a NULL_ROW_ID of a side's filter reads
+ *     as NULL in every column.
+ *   - Inner: the pairs whose key matches and that pass, in hyb_join_hash's order (partition, probe row, build row).
+ *   - Left / Right (the probe side is preserved): the passing pairs; a probe row with key matches but no passing
+ *     candidate emits one (NULL_ROW_ID, probe) row where its pairs would have been; NULL keys and rows without a key
+ *     match emit (NULL_ROW_ID, probe) as in hyb_join_hash.
+ *   - Semi: the probe row once if some candidate passes. AntiNullAsFalse: the probe row if no candidate passes (rows
+ *     without a key match and NULL keys included). AntiNullAsTrue: HYB_ERR_UNSUPPORTED.
+ * predicate_count == 0 is hyb_join_hash: the same result and hyb_join_path. Otherwise the path carries
+ * HYB_JOIN_PATH_SECONDARY and hyb_join_result_output_chunks returns HYB_ERR_UNSUPPORTED for the result (the reference
+ * cuts its slices by probe elements, not by emitted rows). Errors: HYB_ERR_UNSUPPORTED for a string x string pair, more
+ * than HYB_MAX_JOIN_PREDICATES predicates, AntiNullAsTrue, or a side whose RowIDs stand for another table's (the received
+ * tuples of a radix exchange); HYB_ERR_INVALID for a string x numeric pair ("Types of columns cannot be compared"), a
+ * column out of range, a condition other than the six above, or a non-zero `reserved`.
+ */
+#define HYB_MAX_JOIN_PREDICATES 4
+typedef struct hyb_join_predicate {
+  uint32_t build_column_id;
+  uint32_t probe_column_id;
+  int32_t condition; /* HYB_PRED_EQUALS .. HYB_PRED_GREATER_THAN_EQUALS */
+  uint32_t reserved; /* must be 0 */
+} hyb_join_predicate;
+int hyb_join_hash_predicates(hyb_context* context, const hyb_join_side* build, const hyb_join_side* probe, int32_t mode,
+                             int32_t radix_bits, const hyb_join_predicate* predicates, uint32_t predicate_count,
+                             hyb_join_result_t* out_result);
+
 /* out_pair_count: number of emitted rows; out_partition_count: 2^radix_bits. */
 int hyb_join_result_info(hyb_context* context, hyb_join_result_t result, uint64_t* out_pair_count,
                          uint32_t* out_partition_count, int32_t* out_radix_bits);
@@ -975,8 +1010,8 @@ typedef enum hyb_aggregate_path {
 /* The table and kernels of a JoinHash call (hyb_operator_stats::path): one TABLE code | one PROBE code | RERUN.
  * Combinations that cannot occur: a rank table is built only from strictly increasing (so unique) keys and never reruns,
  * and the tile kernels' lean loop reads direct tables only (rank | TILE_LEAN); hash tables never take the span kernels or
- * the lean loop (the lean loop and the span kernels index a direct or rank table); Semi / Anti joins never rerun and
- * never take the span kernels (both serve Inner joins only); TABLE_HASH needs int32 keys on both sides, TABLE_HASH_WIDE
+ * the lean loop (the lean loop and the span kernels index a direct or rank table); Semi / Anti joins rerun only with
+ * secondary predicates and never take the span kernels (both serve Inner joins only); TABLE_HASH needs int32 keys on both sides, TABLE_HASH_WIDE
  * an int64 key on either side; DIRECT_SHIFTED takes the span kernels or the lean loop only for int64 probe keys. */
 typedef enum hyb_join_path {
   HYB_JOIN_PATH_TABLE_RANK = 1,            /* rank table: presence bits + smallest position per 32 key values */
@@ -994,6 +1029,9 @@ typedef enum hyb_join_path {
   HYB_JOIN_PATH_RERUN = 0x100,             /* duplicate build keys: the per-key position lists were built and the probe
                                               ran again on the tile kernels' generic loop; the PROBE code names the first
                                               probe */
+  HYB_JOIN_PATH_SECONDARY = 0x200,         /* hyb_join_hash_predicates with predicates: the tile kernels' generic loop
+                                              evaluated them per candidate (PROBE_TILE); a duplicated build key reruns,
+                                              Semi / Anti joins included */
 } hyb_join_path;
 
 /* Stats of the last operator call made on this context by the calling thread. */

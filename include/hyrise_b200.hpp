@@ -7,6 +7,7 @@
 //     src/lib/operators/abstract_operator.hpp:72-129
 //   TableScan(in, predicate)          table_scan.hpp:23-47         TableScan(context, input, ColumnVsValue / Between / IsNull)
 //   JoinHash(left, right, mode, OperatorJoinPredicate, radix_bits) JoinHash(context, left, right, mode, predicate, radix_bits)
+//   JoinHash(left, right, mode, primary, secondary, radix_bits)    the same with secondary predicates (hyb_join_hash_predicates)
 //     join_hash.hpp:27-39, operator_join_predicate.hpp:16-44         build/probe side selection as join_hash.cpp:139-155
 //   AggregateHash(in, aggregates, groupby_column_ids)             AggregateHash(context, input, aggregates, groupby_column_ids)
 //     aggregate_hash.hpp:86-90, abstract_aggregate_operator.hpp
@@ -669,6 +670,14 @@ class JoinHash : public Operator<JoinOutput> {
       throw std::logic_error("JoinHash only supports equi joins");  // join_hash.cpp:60-63
     }
   }
+  // join_hash.hpp:35: secondary predicates `left <condition> right` after the primary equality (hyb_join_hash_predicates).
+  // Flipped with the inputs when the right input builds (join_hash.cpp:158-165); UnsupportedOnDevice where the library
+  // answers HYB_ERR_UNSUPPORTED (string pairs, AntiNullAsTrue, more than HYB_MAX_JOIN_PREDICATES).
+  JoinHash(OperatorInput left, OperatorInput right, JoinMode mode, OperatorJoinPredicate primary_predicate,
+           std::vector<OperatorJoinPredicate> secondary_predicates, std::optional<int32_t> radix_bits = std::nullopt)
+      : JoinHash(std::move(left), std::move(right), mode, primary_predicate, radix_bits) {
+    _secondary = std::move(secondary_predicates);
+  }
 
  protected:
   std::shared_ptr<const JoinOutput> _on_execute() override {
@@ -683,7 +692,19 @@ class JoinHash : public Operator<JoinOutput> {
     const hyb_join_side& build = left_is_build ? left : right;
     const hyb_join_side& probe = left_is_build ? right : left;
     hyb_join_result_t handle = 0;
-    check(hyb_join_hash(context, &build, &probe, static_cast<int32_t>(_mode), _radix_bits.value_or(-1), &handle));
+    if (_secondary.empty()) {
+      check(hyb_join_hash(context, &build, &probe, static_cast<int32_t>(_mode), _radix_bits.value_or(-1), &handle));
+    } else {
+      std::vector<hyb_join_predicate> adjusted;
+      for (const auto& predicate : _secondary) {
+        const auto [left_column, right_column] = predicate.column_ids;
+        adjusted.push_back(left_is_build ? hyb_join_predicate{left_column, right_column, static_cast<int32_t>(predicate.predicate_condition), 0}
+                                         : hyb_join_predicate{right_column, left_column,
+                                                              static_cast<int32_t>(flip_predicate_condition(predicate.predicate_condition)), 0});
+      }
+      check(hyb_join_hash_predicates(context, &build, &probe, static_cast<int32_t>(_mode), _radix_bits.value_or(-1), adjusted.data(),
+                                     static_cast<uint32_t>(adjusted.size()), &handle));
+    }
     check(hyb_last_operator_stats(context, &performance_data));
     const bool semi_or_anti = _mode == JoinMode::Semi || _mode == JoinMode::AntiNullAsTrue || _mode == JoinMode::AntiNullAsFalse;
     return std::make_shared<JoinOutput>(_left.table->context(), handle, left_is_build, !semi_or_anti);
@@ -693,6 +714,7 @@ class JoinHash : public Operator<JoinOutput> {
   OperatorInput _left, _right;
   JoinMode _mode;
   OperatorJoinPredicate _predicate;
+  std::vector<OperatorJoinPredicate> _secondary;
   std::optional<int32_t> _radix_bits;
 };
 

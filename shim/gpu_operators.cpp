@@ -615,7 +615,8 @@ std::shared_ptr<const Table> try_gpu_expression_scan(const std::shared_ptr<const
 std::shared_ptr<const Table> try_gpu_join_hash(const std::shared_ptr<const Table>& build_table,
                                                const std::shared_ptr<const Table>& probe_table, ColumnID build_column_id,
                                                ColumnID probe_column_id, JoinMode mode, size_t radix_bits,
-                                               bool build_is_left_input) {
+                                               bool build_is_left_input,
+                                               const std::vector<OperatorJoinPredicate>& secondary_predicates) {
   auto* pool = gpu_column_pool();
   if (!pool) {
     return nullptr;
@@ -627,10 +628,19 @@ std::shared_ptr<const Table> try_gpu_join_hash(const std::shared_ptr<const Table
   }
   const auto build = hyb_join_side{build_entry->handle, build_column_id, 0};
   const auto probe = hyb_join_side{probe_entry->handle, probe_column_id, 0};
+  // the secondary predicates arrive adjusted to `build <condition> probe` (join_hash.cpp:158-165)
+  auto predicates = std::vector<hyb_join_predicate>{};
+  for (const auto& predicate : secondary_predicates) {
+    predicates.push_back(hyb_join_predicate{static_cast<uint32_t>(predicate.column_ids.first),
+                                            static_cast<uint32_t>(predicate.column_ids.second),
+                                            static_cast<int32_t>(predicate.predicate_condition), 0});
+  }
   auto result = hyb_join_result_t{};
-  const auto status = hyb_join_hash(pool->context(), &build, &probe, static_cast<int32_t>(mode), static_cast<int32_t>(radix_bits), &result);
+  const auto status = hyb_join_hash_predicates(pool->context(), &build, &probe, static_cast<int32_t>(mode),
+                                               static_cast<int32_t>(radix_bits), predicates.data(),
+                                               static_cast<uint32_t>(predicates.size()), &result);
   if (status == HYB_ERR_UNSUPPORTED) {
-    return nullptr;  // string / float keys, secondary predicates
+    return nullptr;  // string / float keys, string secondary predicates, AntiNullAsTrue with secondary predicates
   }
   Assert(status == HYB_OK, hyb_last_error());
   // The pairs arrive in the order probe() emits them (partition, probe row, build row): one PosList pair per partition, then

@@ -51,7 +51,8 @@ std::shared_ptr<const Table> try_gpu_expression_scan(const std::shared_ptr<const
 std::shared_ptr<const Table> try_gpu_join_hash(const std::shared_ptr<const Table>& build_table,
                                                const std::shared_ptr<const Table>& probe_table, ColumnID build_column_id,
                                                ColumnID probe_column_id, JoinMode mode, size_t radix_bits,
-                                               bool build_is_left_input);
+                                               bool build_is_left_input,
+                                               const std::vector<OperatorJoinPredicate>& secondary_predicates);
 
 // AggregateHash::_on_execute (aggregate_hash.cpp:1180-1372).
 std::shared_ptr<const Table> try_gpu_aggregate_hash(const std::shared_ptr<const Table>& in_table,
