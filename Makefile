@@ -134,6 +134,12 @@ build/sort_check: tests/cpp/sort_check.cpp include/hyrise_b200.hpp include/hyris
 	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/sort_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
 		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
 
+# AggregateOutput::to_table, a HAVING TableScan and a semi JoinHash over it through the mirror on the GPU.
+build/aggregate_table_check: tests/cpp/aggregate_table_check.cpp include/hyrise_b200.hpp include/hyrise_b200.h $(LIB)
+	@mkdir -p build
+	$(CXX) -O1 -std=c++17 -Wall -Wextra -Iinclude -o $@ tests/cpp/aggregate_table_check.cpp -Lhyrise_b200/lib -lhyrise_b200 \
+		-Wl,-rpath,'$$ORIGIN/../hyrise_b200/lib'
+
 clean:
 	rm -rf build $(LIB) $(TPCH_LIB)
 	$(MAKE) -C oracle clean

@@ -180,6 +180,11 @@ class AggregateSortKey(C.Structure):
     _fields_ = [("kind", C.c_int32), ("index", C.c_uint32), ("descending", C.c_int32)]
 
 
+class AggregateOutputColumn(C.Structure):
+    """hyb_aggregate_output_column: kind SORT_KEY_AGGREGATE | SORT_KEY_COLUMN, and the aggregate or column index."""
+    _fields_ = [("kind", C.c_int32), ("index", C.c_uint32)]
+
+
 class DistributedStats(C.Structure):
     _fields_ = [("split_count_ms", C.c_float), ("count_wait_ms", C.c_float), ("push_ms", C.c_float),
                 ("done_wait_ms", C.c_float), ("local_ms", C.c_float), ("finish_ms", C.c_float),
@@ -300,6 +305,7 @@ SYMBOLS = {
     "hyb_aggregate_result_top_k": [_CTX, _U64, _U32, _U32, _I32, _P, C.POINTER(_U32)],
     "hyb_sort": [_CTX, _U64, _U64, C.POINTER(SortColumn), _U32, C.POINTER(_U64)],
     "hyb_aggregate_result_sort": [_CTX, _U64, C.POINTER(AggregateSortKey), _U32, _P],
+    "hyb_aggregate_result_table": [_CTX, _U64, C.POINTER(AggregateOutputColumn), _U32, _U32, C.POINTER(_U64)],
     "hyb_last_operator_stats": [_CTX, C.POINTER(OperatorStats)],
     "hyb_pos_list_device_ptr": [_CTX, _U64, C.POINTER(_P)],
     "hyb_join_result_device_ptrs": [_CTX, _U64, C.POINTER(_P), C.POINTER(_P)],

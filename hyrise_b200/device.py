@@ -13,7 +13,7 @@ import numpy as np
 
 from . import capi
 from .capi import check
-from .storage import NUMPY_TYPES, Table, TableViewHolder
+from .storage import NUMPY_TYPES, Chunk, ColumnDefinition, Segment, Table, TableViewHolder
 
 ROW_ID_DTYPE = np.dtype([("chunk_id", np.uint32), ("chunk_offset", np.uint32)])
 # hyb_dictionary_position: a string MIN / MAX result, entry value_id of chunk chunk_id's dictionary
@@ -478,6 +478,7 @@ class DeviceContext:
         check(self.lib.hyb_context_create(device_index, C.byref(ptr)))
         self.ptr = ptr
         self.device_index = device_index
+        self._kept_sources: dict[int, Table] = {}  # result handle -> host table of a kept aggregate's input
 
     def close(self) -> None:
         if self.ptr:
@@ -653,8 +654,39 @@ class DeviceContext:
         check(self.lib.hyb_aggregate_result_sort(self.ptr, result_handle, array, len(keys), indexes.ctypes.data))
         return indexes[: groups.value]
 
+    def aggregate_table(self, result_handle: int, columns: Sequence[tuple[int, int]],
+                        chunk_size: int = capi.DEFAULT_CHUNK_SIZE) -> DeviceTable:
+        """hyb_aggregate_result_table on a result kept alive with aggregate_hash(..., keep_result=True): the result as a
+        table of the pool, column c = columns[c], (capi.SORT_KEY_AGGREGATE, aggregate index) or (capi.SORT_KEY_COLUMN,
+        column of the aggregated table at the representative RowIDs). Every operator takes it like an uploaded table.
+        Its host_table holds the derived schema and chunking only; the values live on the device."""
+        array = (capi.AggregateOutputColumn * max(len(columns), 1))(*[capi.AggregateOutputColumn(kind, index)
+                                                                      for kind, index in columns])
+        handle = C.c_uint64()
+        check(self.lib.hyb_aggregate_result_table(self.ptr, result_handle, array, len(columns), chunk_size,
+                                                  C.byref(handle)))
+        groups, immediate = C.c_uint64(), C.c_int32()
+        check(self.lib.hyb_aggregate_result_info(self.ptr, result_handle, C.byref(groups), C.byref(immediate)))
+        source = self._kept_sources.get(result_handle)
+        definitions = []
+        for position, (kind, index) in enumerate(columns):
+            if kind == capi.SORT_KEY_AGGREGATE:
+                value_type = C.c_int32()
+                check(self.lib.hyb_aggregate_result_values(self.ptr, result_handle, index, None, None, C.byref(value_type)))
+                definitions.append(ColumnDefinition(f"aggregate_{index}", value_type.value, True))
+            else:
+                definitions.append(ColumnDefinition(source.column_definitions[index].name,
+                                                    source.column_definitions[index].data_type, True))
+        host_table = Table(definitions, target_chunk_size=chunk_size)
+        for begin in range(0, groups.value, chunk_size):
+            rows = min(chunk_size, groups.value - begin)
+            host_table.chunks.append(Chunk([Segment(capi.ENC_UNENCODED, definition.data_type, rows)
+                                            for definition in definitions]))
+        return DeviceTable(self, handle.value, host_table, None)
+
     def free_aggregate_result(self, result_handle: int) -> None:
         check(self.lib.hyb_aggregate_result_free(self.ptr, result_handle))
+        self._kept_sources.pop(result_handle, None)
 
     def set_string_order(self, table: DeviceTable, column_id: int, ranks: np.ndarray | None = None) -> None:
         """hyb_table_set_string_order: attach the order ranks MIN / MAX over a string column need; computed from the host
@@ -718,6 +750,8 @@ class DeviceContext:
         definitions = table.host_table.column_definitions
         any_types = {index: definitions[aggregate.expression.nodes[0][1]].data_type
                      for index, aggregate in enumerate(aggregates) if aggregate.function == capi.AGG_ANY}
+        if keep_result:  # aggregate_table types its COLUMN outputs from the aggregated table's schema
+            self._kept_sources[handle.value] = table.host_table
         return self._collect_aggregate(handle.value, len(aggregates), keep_result, any_types)
 
     def last_stats(self) -> capi.OperatorStats:

@@ -980,6 +980,41 @@ typedef struct hyb_aggregate_sort_key {
 int hyb_aggregate_result_sort(hyb_context* context, hyb_aggregate_result_t result, const hyb_aggregate_sort_key* keys,
                               uint32_t key_count, uint32_t* out_group_indexes);
 
+/*
+ * An aggregate result as an ordinary table of the pool: the reference's AggregateHash output (aggregate values in a
+ * materialised Data table, aggregate_hash.cpp:1301-1324; GROUP BY columns through the representative rows, :421-537), so a
+ * HAVING is hyb_table_scan (or any other scan) over it, an IN subquery a semi join onto it, and a view's aggregate, join
+ * or sort takes it like any stored table.
+ *   - Row g of the table is group g of the result, in the result's group order, at RowID {g / chunk_size, g % chunk_size};
+ *     every chunk but the last holds chunk_size rows. A result without groups gives a table without chunks whose column
+ *     types are set, so every operator over it returns its empty result.
+ *   - Column c is columns[c]: kind HYB_SORT_KEY_AGGREGATE = aggregate `index` of the result, exactly what
+ *     hyb_aggregate_result_values reports (its type, bit-identical values including NaN payloads and -0.0, its NULLs);
+ *     kind HYB_SORT_KEY_COLUMN = the aggregated table's numeric column `index`, any encoding, decoded at the group's
+ *     representative RowID (what write_groupby_output's ReferenceSegments show): NULL where that row is NULL (the NULL
+ *     group) or the RowID is NULL_ROW_ID (the synthesised row of an empty input without GROUP BY). ANY is taken this way.
+ *   - Every segment is an UNENCODED value segment in table-owned device memory. An aggregate column carries a NULL vector
+ *     when one of its groups is NULL, a COLUMN column always does.
+ *   - The table owns its buffers (hyb_table_drop frees them) and depends on neither the result nor the aggregated table:
+ *     either may be freed or dropped first. The result stays host-resident; its values are uploaded once per call.
+ * HYB_ERR_UNSUPPORTED: a string MIN / MAX, a STRING column (rows from different source chunks share no dictionary),
+ * 2^32 - 1 or more groups. HYB_ERR_INVALID: NULL pointers, no columns, chunk_size 0, an unknown result, an unknown kind,
+ * an index out of range, ANY as an aggregate column (take it through HYB_SORT_KEY_COLUMN), a COLUMN column after the
+ * aggregated table was dropped or with a representative RowID outside it (a distributed result's global RowIDs).
+ * hyb_operator_stats: input_rows = output_rows = group_count; kernel_launches = 1 when a COLUMN column and a group exist
+ * (aggregate_table_gather_kernel, all COLUMN columns in one launch), else 0; algorithmic_bytes = bytes uploaded
+ * (aggregate values and NULL bytes, the representative RowIDs when gathered) + source column bytes gathered (element size
+ * per group and COLUMN column) + bytes the gather writes (element size + 1 NULL byte per group and COLUMN column);
+ * path = 0.
+ */
+typedef struct hyb_aggregate_output_column {
+  int32_t kind; /* HYB_SORT_KEY_AGGREGATE | HYB_SORT_KEY_COLUMN, the vocabulary of hyb_aggregate_sort_key */
+  uint32_t index;
+} hyb_aggregate_output_column;
+int hyb_aggregate_result_table(hyb_context* context, hyb_aggregate_result_t result,
+                               const hyb_aggregate_output_column* columns, uint32_t column_count, uint32_t chunk_size,
+                               hyb_table_t* out_table);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Instrumentation (fills the reference's performance_data, operators/operator_performance_data.hpp:46-97)
  * ---------------------------------------------------------------------------------------------------------------- */

@@ -217,6 +217,8 @@ class DeviceTable {
   DeviceTable(std::shared_ptr<DeviceContext> context, const BinaryTable& file) : _context(std::move(context)) {
     check(hyb_table_upload_binary(_context->get(), file.get(), &_handle));
   }
+  // Takes ownership of a table the library created (AggregateOutput::to_table).
+  DeviceTable(std::shared_ptr<DeviceContext> context, hyb_table_t handle) : _context(std::move(context)), _handle(handle) {}
   ~DeviceTable() { hyb_table_drop(_context->get(), _handle); }
   DeviceTable(const DeviceTable&) = delete;
   DeviceTable& operator=(const DeviceTable&) = delete;
@@ -849,6 +851,16 @@ class AggregateOutput {
     std::vector<uint32_t> out(group_count());
     check(hyb_aggregate_result_sort(_context->get(), _handle, keys.data(), static_cast<uint32_t>(keys.size()), out.data()));
     return out;
+  }
+  // The output as a stored table (hyb_aggregate_result_table): column c = columns[c], an aggregate or a column of the
+  // aggregated table at the representative rows. A HAVING is a TableScan over it, an IN subquery a semi JoinHash onto
+  // it. The table lives on after this output and the aggregated table are gone.
+  std::shared_ptr<DeviceTable> to_table(const std::vector<hyb_aggregate_output_column>& columns,
+                                        uint32_t chunk_size = HYB_DEFAULT_CHUNK_SIZE) const {
+    hyb_table_t table = 0;
+    check(hyb_aggregate_result_table(_context->get(), _handle, columns.data(), static_cast<uint32_t>(columns.size()),
+                                     chunk_size, &table));
+    return std::make_shared<DeviceTable>(_context, table);
   }
   // A string MIN / MAX: per group the string (std::nullopt for NULL), read from the table the aggregate ran on.
   std::vector<std::optional<std::string>> strings(uint32_t aggregate_index, const BinaryTable& table, uint32_t column) const {
